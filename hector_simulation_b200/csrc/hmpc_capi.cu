@@ -155,7 +155,9 @@ struct hmpc_ctx {
   cudaStream_t gstream = nullptr;  // the gather runs here, behind `solved`, beside the next tick
   cudaEvent_t solved = nullptr, gathered[2] = {nullptr, nullptr};
   int* d_ws = nullptr;             // [max_batch][WS_STATE_INTS] working sets of the previous tick (closed-loop warm start)
-  int warm_start = 1;              // hmpc_rollout_device proposes them to the next tick (HMPC_WARM_START=0: cold start every tick)
+  int warm_start = 1;              // the warm calls propose them to the next tick (HMPC_WARM_START=0: cold start every tick)
+  int* d_shift = nullptr;          // [max_batch] per-robot shifts of hmpc_solve_batch_warm (staged copy)
+  int* h_shift = nullptr;          // pinned [max_batch] the same, also read mapped by the zero-copy and in-place modes
   int lockstep = 1;                // waves of a multi-wave launch start together (HMPC_LOCKSTEP=0: free-running, for A/B runs)
   double kappa_max = 1.5e5;  // conditioning limit of the fp64 sweep inversion (HMPC_KAPPA_MAX; see the kernel's stage 5)
   int block_min = 2;     // later rounds need at least this many entering rows (HMPC_BLOCK_MIN, A/B knob)
@@ -519,6 +521,8 @@ HMPC_EXTERNC void hmpc_destroy(hmpc_ctx* c)
   if (c->d_cls) cudaFree(c->d_cls);
   shard_release(c);
   if (c->d_ws) cudaFree(c->d_ws);
+  if (c->d_shift) cudaFree(c->d_shift);
+  if (c->h_shift) cudaFreeHost(c->h_shift);
   if (c->d_states) cudaFree(c->d_states);
   if (c->h_states) cudaFreeHost(c->h_states);
   if (c->h_rec) cudaFreeHost(c->h_rec);
@@ -572,6 +576,8 @@ HMPC_EXTERNC hmpc_ctx* hmpc_create(int max_batch, int horizon, int device)
           cuda_fail(cudaMalloc(&c->d_lists, (size_t)NCHUNK * (4 + 3 * (size_t)max_batch) * sizeof(int)), "cudaMalloc lists") ||
           cuda_fail(cudaMalloc(&c->d_ws, (size_t)max_batch * hmpc::WS_STATE_INTS * sizeof(int)), "cudaMalloc working sets") ||
           cuda_fail(cudaMemset(c->d_ws, 0, (size_t)max_batch * hmpc::WS_STATE_INTS * sizeof(int)), "cudaMemset working sets") ||
+          cuda_fail(cudaMalloc(&c->d_shift, (size_t)max_batch * sizeof(int)), "cudaMalloc shifts") ||
+          cuda_fail(cudaMallocHost(&c->h_shift, (size_t)max_batch * sizeof(int)), "cudaMallocHost shifts") ||
           cuda_fail(cudaMalloc(&c->d_cls, (size_t)NCHUNK * (8 + 2 * (size_t)max_batch) * sizeof(int)), "cudaMalloc class lists") ||
           cuda_fail(cudaMemset(c->d_cls, 0, (size_t)NCHUNK * (8 + 2 * (size_t)max_batch) * sizeof(int)), "cudaMemset class lists") ||
           cuda_fail(cudaMalloc(&c->d_status, (size_t)max_batch * 4), "cudaMalloc status") ||
@@ -621,7 +627,7 @@ long long* g_dbg_clk = nullptr;  // profiling hook (hmpc_debug_set_clock_buffer)
 // classification pre-pass + one launch per class, all enqueued on `st`
 int enqueue_solve(hmpc_ctx* c, const void* d_records, int B, float* d_wrench32, double* d_wrench64, int* d_status,
                   cudaStream_t st, int slot = 0, float* d_tau = nullptr, int* d_ws = nullptr, int ws_shift = 0, bool ws_read = false,
-                  const update_data_t* raw = nullptr)
+                  const update_data_t* raw = nullptr, const int* ws_shifts = nullptr)
 {
   if (B > c->max_batch) { g_err = "batch exceeds the context's capacity"; return HMPC_ERR_ARG; }
   CK(cudaSetDevice(c->device));
@@ -642,6 +648,7 @@ int enqueue_solve(hmpc_ctx* c, const void* d_records, int B, float* d_wrench32, 
     ka.warm_start = (d_ws && ws_read) ? 1 : 0;
     ka.ws_state = d_ws;
     ka.ws_shift = ws_shift;
+    ka.ws_shifts = ws_shifts;
     ka.list = (i == 0) ? nullptr : lists + (size_t)i * c->max_batch;
     ka.split_nb = (i == 0) ? k.nb_hi : -1;
     ka.counts_next = (i == 0) ? counts_next : nullptr;
@@ -660,6 +667,15 @@ int enqueue_solve(hmpc_ctx* c, const void* d_records, int B, float* d_wrench32, 
     CK(launch_class(k, ka, grid, st, pdl));
   }
   return HMPC_OK;
+}
+
+// the warm-started device-resident solve: robot i's proposal is its set in the context's d_ws, moved d_shift[i] steps
+// (d_shift NULL: every robot one step, the closed loop's tick); HMPC_WARM_START=0 makes it a cold solve
+int enqueue_solve_warm(hmpc_ctx* c, const void* d_records, int B, float* d_wrench, int* d_status, cudaStream_t st, float* d_tau,
+                       const int* d_shift)
+{
+  return enqueue_solve(c, d_records, B, d_wrench, nullptr, d_status, st, 0, d_tau, c->warm_start ? c->d_ws : nullptr, 1, true,
+                       nullptr, d_shift);
 }
 }  // namespace
 
@@ -686,7 +702,7 @@ void classify_host(const hmpc_ctx* c, const unsigned char* gait0, size_t gait_st
 
 int enqueue_solve_hostlists(hmpc_ctx* c, const void* d_records, int nb, int* h_block, float* d_wrench32, int* d_status,
                             cudaStream_t st, int slot, float* d_tau, bool zero_copy, const update_data_t* raw = nullptr,
-                            double* wrench64 = nullptr)
+                            double* wrench64 = nullptr, int* d_ws = nullptr, const int* ws_shifts = nullptr)
 {
   int* d_block = c->d_lists + (size_t)slot * (4 + 3 * (size_t)c->max_batch);
   const int n0 = h_block[0], n1 = h_block[1];
@@ -705,11 +721,63 @@ int enqueue_solve_hostlists(hmpc_ctx* c, const void* d_records, int nb, int* h_b
     ka.raw_records = reinterpret_cast<const unsigned char*>(raw);
     ka.wrench64 = wrench64;
     ka.tau = d_tau;
-    ka.warm_start = 0;
+    ka.warm_start = d_ws ? 1 : 0;
+    ka.ws_state = d_ws;
+    ka.ws_shift = 1;
+    ka.ws_shifts = ws_shifts;
     ka.list = d_block + 4 + (size_t)i * c->max_batch;
     ka.counts = d_block;
     ka.cls = i;
     ka.esc_list = nullptr;  // overflow is handled by the caller's retry
+    ka.split_nb = -1;
+    ka.nb_cap = k.nb_cap;
+    ka.qmax = k.qmax;
+    ka.tcap = k.tcap;
+    ka.L = k.L;
+    ka.dbg_clk = g_dbg_clk;
+    const int grid = cnt < k.grid_cap ? cnt : k.grid_cap;
+    CK(launch_class(k, ka, grid, st));
+  }
+  return HMPC_OK;
+}
+
+// Working-set overflow in a host-list launch (rare: massively degenerate optima).  Only the instances that overflowed are
+// solved again, from where the device-resident chain would have taken them: class 0's by class 1, class 1's by class 2,
+// with escalation from the one to the other.  The rest of the chunk keeps its results and its recorded working sets, and an
+// instance that overflowed kept its proposal (the kernel does not record a set for it), so results, statuses and working
+// sets are those of the device-resident path.  `h_block` holds the chunk's class lists and is reused for the retry's.
+int enqueue_overflow_retry(hmpc_ctx* c, const void* d_records, int nb, int* h_block, const int* h_status, float* d_wrench32,
+                           int* d_status, cudaStream_t st, int slot, float* d_tau, int* d_ws, const int* ws_shifts)
+{
+  const size_t mb = c->max_batch;
+  std::vector<char> was_cls1(nb, 0);
+  for (int j = 0; j < h_block[1]; j++) was_cls1[h_block[4 + mb + j]] = 1;
+  int n[3] = {0, 0, 0};
+  for (int i = 0; i < nb; i++) {
+    if (HMPC_STATUS_CODE(h_status[i]) != hmpc::ST_WS_CAP) continue;
+    const int next = was_cls1[i] ? 2 : 1;
+    if (next < c->ncls) h_block[4 + next * mb + n[next]++] = i;  // (class 1 as the last class: its overflow is final)
+  }
+  h_block[0] = 0;
+  h_block[1] = n[1];
+  h_block[2] = n[2];
+  h_block[3] = 0;
+  int* d_block = c->d_lists + (size_t)slot * (4 + 3 * mb);
+  CK(cudaMemcpyAsync(d_block, h_block, (4 + 2 * mb + n[2]) * sizeof(int), cudaMemcpyHostToDevice, st));
+  for (int i = 1; i < c->ncls; i++) {
+    const int cnt = (i == 1) ? n[1] : n[1] + n[2];  // class 2's list grows by class 1's escalations
+    if (cnt == 0) continue;
+    const ClassCfg& k = c->cls[i];
+    hmpc::KernelArgs ka = base_args(c, d_records, nb, d_wrench32, d_status);
+    ka.tau = d_tau;
+    ka.warm_start = d_ws ? 1 : 0;
+    ka.ws_state = d_ws;
+    ka.ws_shift = 1;
+    ka.ws_shifts = ws_shifts;
+    ka.list = d_block + 4 + i * mb;
+    ka.counts = d_block;
+    ka.cls = i;
+    ka.esc_list = (i + 1 < c->ncls) ? d_block + 4 + (i + 1) * mb : nullptr;
     ka.split_nb = -1;
     ka.nb_cap = k.nb_cap;
     ka.qmax = k.qmax;
@@ -771,6 +839,15 @@ HMPC_EXTERNC int hmpc_solve_device_ex(hmpc_ctx* c, const void* d_records, int B,
   return enqueue_solve(c, d_records, B, d_wrench, nullptr, d_status, static_cast<cudaStream_t>(stream), 0, d_tau);
 }
 
+HMPC_EXTERNC int hmpc_solve_device_warm(hmpc_ctx* c, const void* d_records, int B, float* d_wrench, int* d_status, float* d_tau,
+                                        const int* d_shift, void* stream)
+{
+  if (!c || !d_records || !d_wrench || !d_status || B < 0) { g_err = "hmpc_solve_device_warm: bad argument"; return HMPC_ERR_ARG; }
+  if (B == 0) return HMPC_OK;
+  if (int rc = check_device_records(c, d_records, B, "hmpc_solve_device_warm")) return rc;
+  return enqueue_solve_warm(c, d_records, B, d_wrench, d_status, static_cast<cudaStream_t>(stream), d_tau, d_shift);
+}
+
 HMPC_EXTERNC int hmpc_assemble_device(hmpc_ctx* c, const void* d_records, int B, float* d_H, float* d_g,
                                       float* d_Fblk, float* d_lb, float* d_ub, void* stream)
 {
@@ -803,7 +880,7 @@ HMPC_EXTERNC int hmpc_assemble_device(hmpc_ctx* c, const void* d_records, int B,
 }
 
 static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_state_t* sin, int B, double* wrench_out,
-                            double* tau_out, int* status, double dtMPC = 0.0);
+                            double* tau_out, int* status, double dtMPC = 0.0, bool warm = false, const int* shift = nullptr);
 
 HMPC_EXTERNC int hmpc_solve_batch(hmpc_ctx* c, const update_data_t* in, int B, double* wrench_out, int* status)
 {
@@ -814,6 +891,13 @@ HMPC_EXTERNC int hmpc_solve_batch_ex(hmpc_ctx* c, const update_data_t* in, int B
                                      int* status)
 {
   return solve_batch_impl(c, in, nullptr, B, wrench_out, tau_out, status);
+}
+
+HMPC_EXTERNC int hmpc_solve_batch_warm(hmpc_ctx* c, const update_data_t* in, int B, double* wrench_out, double* tau_out,
+                                       int* status, const int* shift)
+{
+  if (!in) { g_err = "hmpc_solve_batch_warm: bad argument (null records)"; return HMPC_ERR_ARG; }
+  return solve_batch_impl(c, in, nullptr, B, wrench_out, tau_out, status, 0.0, true, shift);
 }
 
 static_assert(sizeof(hmpc_state_t) == 352 && offsetof(hmpc_state_t, gait) == 39 * 8, "hmpc_state_t layout (hmpc_prepare_kernel)");
@@ -916,7 +1000,7 @@ HMPC_EXTERNC int hmpc_rollout_device(hmpc_ctx* c, hmpc_state_t* d_states, hmpc_r
     if (d_record_log)
       CK(cudaMemcpyAsync(static_cast<unsigned char*>(d_record_log) + (size_t)t * B * c->rec_stride, c->d_rec,
                          (size_t)B * c->rec_stride, cudaMemcpyDeviceToDevice, st));
-    rc = enqueue_solve(c, c->d_rec, B, dw, nullptr, ds, st, 0, nullptr, c->warm_start ? c->d_ws : nullptr, 1, true);
+    rc = enqueue_solve_warm(c, c->d_rec, B, dw, ds, st, nullptr, nullptr);
     if (rc != HMPC_OK) return rc;
     hmpc::hmpc_advance_kernel<<<(B + 63) / 64, 64, 0, st>>>(reinterpret_cast<unsigned char*>(d_states),
                                                             reinterpret_cast<unsigned char*>(d_loop), B, c->horizon, dtMPC, dw, ds,
@@ -957,7 +1041,7 @@ HMPC_EXTERNC int hmpc_solve_batch_states(hmpc_ctx* c, const hmpc_state_t* in, in
 }
 
 static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_state_t* sin, int B, double* wrench_out,
-                            double* tau_out, int* status, double dtMPC)
+                            double* tau_out, int* status, double dtMPC, bool warm, const int* shift)
 {
   if (!c || (!in && !sin) || !wrench_out || B < 0 || B > c->max_batch) {
     g_err = "hmpc_solve_batch: bad argument (null pointer or batch > capacity)";
@@ -984,6 +1068,13 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
   static const int zc_env = getenv("HMPC_ZEROCOPY") ? atoi(getenv("HMPC_ZEROCOPY")) : -1;
   const bool zc = zc_env >= 0 ? (zc_env != 0) : (B <= 1536);
   if (zc && nch_env < 1) nch = 1;
+  // warm start (hmpc_solve_batch_warm): the context's working sets, per-robot shifts from the pinned copy of `shift`
+  int* ws = (warm && c->warm_start) ? c->d_ws : nullptr;
+  const int* hsh = nullptr;
+  if (ws && shift) {
+    memcpy(c->h_shift, shift, (size_t)B * sizeof(int));
+    hsh = c->h_shift;
+  }
   // in-place mode: records, wrenches and status all live in buffers the caller registered (hmpc_pin_host_buffer):
   // the kernels gather the live bytes of every update_data_t over PCIe and store double results where the caller
   // wants them — the call is host classification + launches + one synchronize
@@ -992,7 +1083,7 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
     // the device-resident chain on the caller's records: class 0 classifies on the way, overflow escalates on the device
     int* ds = status ? status : reinterpret_cast<int*>(c->h_out + (size_t)c->max_batch * nw * 4);
     float* dt_ = tau_out ? reinterpret_cast<float*>(c->h_out + (size_t)c->max_batch * (nw * 4 + 4)) : nullptr;
-    int rc = enqueue_solve(c, nullptr, B, c->shard_out, wrench_out, ds, c->stream, 0, dt_, nullptr, 0, false, in);
+    int rc = enqueue_solve(c, nullptr, B, c->shard_out, wrench_out, ds, c->stream, 0, dt_, ws, 1, ws != nullptr, in, hsh);
     if (rc != HMPC_OK) return rc;
     if (c->shard_out) {
       CK(cudaEventRecord(c->solved, c->stream));
@@ -1050,7 +1141,16 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
     int* hblk = c->h_cls + (size_t)k * (4 + 3 * (size_t)c->max_batch);
     if (sin) classify_host(c, sin[b0].gait, sizeof(hmpc_state_t), nb, hblk);
     else classify_host(c, in[b0].gait, sizeof(update_data_t), nb, hblk);
-    rc = enqueue_solve_hostlists(c, rbase + (size_t)b0 * c->rec_stride, nb, hblk, dw, ds, sts[k], k, dt_, zc);
+    int* ws_k = ws ? ws + (size_t)b0 * hmpc::WS_STATE_INTS : nullptr;
+    const int* sh_k = nullptr;
+    if (hsh && zc) {
+      sh_k = hsh + b0;  // mapped, like the records and lists of this mode
+    } else if (hsh) {
+      CK(cudaMemcpyAsync(c->d_shift + b0, hsh + b0, (size_t)nb * sizeof(int), cudaMemcpyHostToDevice, sts[k]));
+      sh_k = c->d_shift + b0;
+    }
+    rc = enqueue_solve_hostlists(c, rbase + (size_t)b0 * c->rec_stride, nb, hblk, dw, ds, sts[k], k, dt_, zc, nullptr, nullptr,
+                                 ws_k, sh_k);
     if (rc != HMPC_OK) return rc;
     if (!zc) CK(cudaMemcpyAsync(c->h_out + ooff, c->d_out + ooff, obytes, cudaMemcpyDeviceToHost, sts[k]));
     if (trace) tr[ntr++] = now();
@@ -1062,7 +1162,7 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
     CK(cudaStreamSynchronize(sts[k]));
     if (trace) tr[ntr++] = now();
     const size_t ooff = (size_t)b0 * (nw * 4 + 4 + 40);
-    {  // working-set overflow (rare, massively degenerate optima): redo the chunk through the escalating device path
+    {  // working-set overflow (rare, massively degenerate optima): the overflowed instances escalate (enqueue_overflow_retry)
       const int* hs = reinterpret_cast<const int*>(c->h_out + ooff + (size_t)nb * nw * 4);
       bool overflow = false;
       for (int i = 0; i < nb; i++) overflow |= (HMPC_STATUS_CODE(hs[i]) == hmpc::ST_WS_CAP);
@@ -1072,7 +1172,10 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
         int* ds = reinterpret_cast<int*>(obase + ooff + (size_t)nb * nw * 4);
         float* dt_ = tau_out ? reinterpret_cast<float*>(obase + ooff + (size_t)nb * (nw * 4 + 4)) : nullptr;
         const unsigned char* rbase = (zc && !sin) ? c->h_rec : c->d_rec;
-        int rc = enqueue_solve(c, rbase + (size_t)b0 * c->rec_stride, nb, dw, nullptr, ds, sts[k], k, dt_);
+        int* hblk = c->h_cls + (size_t)k * (4 + 3 * (size_t)c->max_batch);
+        const int* sh_k = hsh ? (zc ? hsh : c->d_shift) + b0 : nullptr;  // where the first pass read them
+        int rc = enqueue_overflow_retry(c, rbase + (size_t)b0 * c->rec_stride, nb, hblk, hs, dw, ds, sts[k], k, dt_,
+                                        ws ? ws + (size_t)b0 * hmpc::WS_STATE_INTS : nullptr, sh_k);
         if (rc != HMPC_OK) return rc;
         if (!zc)
           CK(cudaMemcpyAsync(c->h_out + ooff, c->d_out + ooff, (size_t)nb * (nw * 4 + 4 + (tau_out ? 40 : 0)),
@@ -1131,6 +1234,7 @@ int g_soln_len = 0;
 int g_has_solved = 0;
 int g_ref_rc = HMPC_OK;       // result of the last update_problem_data (hmpc_reference_last_rc)
 bool g_ref_failing = false;   // inside an episode of failing ticks (the message is printed once per episode)
+bool g_ref_warm = false;      // hmpc_reference_set_warm_start: update_problem_data proposes the previous tick's working set
 
 [[noreturn]] void die(const char* where)
 {
@@ -1168,8 +1272,14 @@ HMPC_EXTERNC void setup_problem(double dt, int horizon, double mu, double f_max)
   s.mu = (float)mu;
   s.f_max = (float)f_max;
   s.horizon = horizon;
+  // the reference's caller sets the same problem up before every tick; a different QP (dt, f_max) forgets the warm start's
+  // working set (a new context — another horizon — starts without one)
+  if (s.dt != g_ctx->setup.dt || s.f_max != g_ctx->setup.f_max)
+    if (hmpc_reset_warm_start(g_ctx, g_ctx->stream) != HMPC_OK) die("setup_problem");
   hmpc_set_problem(g_ctx, &s);
 }
+
+HMPC_EXTERNC void hmpc_reference_set_warm_start(int on) { g_ref_warm = on != 0; }
 
 HMPC_EXTERNC void update_problem_data(double* p, double* v, double* q, double* w, double* r, double* joint_angles,
                                       double yaw, double* weights, double* state_trajectory, double* Alpha_K,
@@ -1186,7 +1296,8 @@ HMPC_EXTERNC void update_problem_data(double* p, double* v, double* q, double* w
   for (int i = 0; i < 12; i++) { ref_update().weights[i] = (float)weights[i]; ref_update().Alpha_K[i] = (float)Alpha_K[i]; }
   for (int i = 0; i < 12 * N; i++) ref_update().traj[i] = (float)state_trajectory[i];
   for (int i = 0; i < 2 * N; i++) ref_update().gait[i] = (unsigned char)gait[i];
-  int rc = hmpc_solve_batch(g_ctx, &g_blk->update, 1, g_blk->soln, &g_blk->status);
+  int rc = g_ref_warm ? hmpc_solve_batch_warm(g_ctx, &g_blk->update, 1, g_blk->soln, nullptr, &g_blk->status, nullptr)
+                      : hmpc_solve_batch(g_ctx, &g_blk->update, 1, g_blk->soln, &g_blk->status);
   g_ref_rc = rc;
   if (rc == HMPC_ERR_NOT_CONVERGED) printf("failed to solve!\n");  // SolverMPC.cpp:714-715 (status word: hmpc_reference_last_status())
   else if (rc != HMPC_OK) {

@@ -159,7 +159,8 @@ struct KernelArgs {
   int block_min;                 // rounds after the first run only with at least this many entering rows
   double kappa_max;              // conditioning limit of the sweep inversion: max_i H_ii (H^-1)_ii beyond it -> ST_NOT_SPD
   int warm_start;                // 1: propose the working set in `ws_state` (previous tick) to the block start
-  int ws_shift;                  // MPC steps the horizon moved since that tick (the closed loop: 1)
+  int ws_shift;                  // MPC steps the horizon moved since that tick (the closed loop: 1); < 0: no history
+  const int* ws_shifts;          // [batch] the same per robot (overrides ws_shift), or nullptr
   int* ws_state;                 // [batch][WS_STATE_INTS] persistent working sets, read (warm_start) and written back; or nullptr
   float* wrench;                 // [batch][12N] float results, or nullptr
   double* wrench64;              // [batch][12N] double results, or nullptr
@@ -1680,12 +1681,13 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
       if (ka.warm_start && ka.ws_state) {
         const int* ws = ka.ws_state + (size_t)inst * WS_STATE_INTS;
         const int cnt = ws[0];
-        if (cnt > 0 && cnt < WS_STATE_INTS) {
+        const int shift = ka.ws_shifts ? ka.ws_shifts[inst] : ka.ws_shift;  // < 0 (e.g. a reset robot): a cold start
+        if (shift >= 0 && cnt > 0 && cnt < WS_STATE_INTS) {
           if (tid < 16) wmark[tid] = 0u;
           __syncthreads();
           if (tid < cnt) {
             const int ent = ws[1 + tid];
-            const int sl = (ent >> 8) - 2 * ka.ws_shift;  // (step, leg): one MPC step later it sits one step earlier
+            const int sl = (ent >> 8) - 2 * shift;  // (step, leg): one MPC step later it sits one step earlier
             if (sl >= 0 && sl < 2 * N) {
               const int kb = sl_blk[sl];
               if (kb >= 0) {
@@ -2147,8 +2149,10 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
       __syncthreads();
     }
 
-    // working set for the next tick (closed loop): (step, leg) and normal index of every active row
-    if (ka.ws_state && wid == 0) {
+    // working set for the next tick (closed loop): (step, leg) and normal index of every active row.  An instance that
+    // overflowed this class's capacity is solved again (by the next class, or the host path's retry) from the same
+    // proposal: it keeps the one it has.
+    if (ka.ws_state && wid == 0 && code != ST_WS_CAP) {
       int* ws = ka.ws_state + (size_t)inst * WS_STATE_INTS;
       const unsigned am = (code == ST_OK && qmax <= 31) ? amask[0] : 0u;
       if ((am >> lane) & 1u) {

@@ -29,6 +29,7 @@ EXPORTS = [
     "hmpc_shard_unique_id", "hmpc_shard_init", "hmpc_solve_batch_sharded", "hmpc_shard_wait",
     "hmpc_pin_host_buffer", "hmpc_unpin_host_buffer", "hmpc_swing_device",
     "hmpc_reference_last_status", "hmpc_reference_last_rc",
+    "hmpc_solve_device_warm", "hmpc_solve_batch_warm", "hmpc_reference_set_warm_start",
 ]
 
 SETUP_DTYPE = np.dtype([("dt", "<f4"), ("mu", "<f4"), ("f_max", "<f4"), ("horizon", "<i4")], align=True)
@@ -106,6 +107,12 @@ def lib() -> ctypes.CDLL:
         L.hmpc_swing_device.restype = ctypes.c_int
         L.hmpc_class_config.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
         L.hmpc_class_config.restype = ctypes.c_int
+        L.hmpc_solve_device_warm.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 5
+        L.hmpc_solve_device_warm.restype = ctypes.c_int
+        L.hmpc_solve_batch_warm.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 4
+        L.hmpc_solve_batch_warm.restype = ctypes.c_int
+        L.hmpc_reference_set_warm_start.argtypes = [ctypes.c_int]
+        L.hmpc_reference_set_warm_start.restype = None
         _lib = L
     return _lib
 
@@ -154,6 +161,12 @@ def reference_last_status() -> int:
 def reference_last_rc() -> int:
     """Result of the last update_problem_data: 0, HMPC_ERR_NOT_CONVERGED, or the error the tick failed with."""
     return lib().hmpc_reference_last_rc()
+
+
+def reference_set_warm_start(on: bool) -> None:
+    """update_problem_data proposes the previous call's working set, moved one step (hmpc_reference_set_warm_start);
+    off by default, like the reference's cold start."""
+    lib().hmpc_reference_set_warm_start(1 if on else 0)
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -265,6 +278,30 @@ class BatchedMPC:
                allow_not_converged=not strict)
         return wrench, status
 
+    def solve_batch_warm(self, records: np.ndarray, shift=None, torques: bool = False, strict: bool = True, out=None):
+        """solve_batch warm-started from each robot's working set of its last warm call (hmpc_solve_batch_warm).
+        `shift` int32 [B]: steps robot i's horizon moved since then (None: all 1; 0: same horizon; < 0: no history).
+        -> (wrench, status), or (wrench, tau, status) with torques=True."""
+        if records.dtype != UPDATE_DTYPE or not records.flags.c_contiguous:
+            records = np.ascontiguousarray(records, dtype=UPDATE_DTYPE)
+        B = records.shape[0]
+        if out is not None:
+            wrench, status = out
+            assert wrench.dtype == np.float64 and wrench.shape == (B, 12 * self.horizon) and wrench.flags.c_contiguous
+            assert status.dtype == np.int32 and status.shape == (B,)
+        else:
+            wrench = np.zeros((B, 12 * self.horizon), dtype=np.float64)
+            status = np.zeros(B, dtype=np.int32)
+        tau = np.zeros((B, 10), dtype=np.float64) if torques else None
+        if shift is not None:
+            shift = np.ascontiguousarray(shift, dtype=np.int32)
+            assert shift.shape == (B,)
+        _check(lib().hmpc_solve_batch_warm(self._h, records.ctypes.data, B, wrench.ctypes.data,
+                                           tau.ctypes.data if torques else None, status.ctypes.data,
+                                           shift.ctypes.data if shift is not None else None),
+               allow_not_converged=not strict)
+        return (wrench, tau, status) if torques else (wrench, status)
+
     def solve_batch_torques(self, records: np.ndarray, strict: bool = True):
         """Host path with the leg-controller epilogue: -> (wrench [B,12N], tau [B,10], status [B])."""
         records = np.ascontiguousarray(records, dtype=UPDATE_DTYPE)
@@ -361,6 +398,16 @@ class BatchedMPC:
         st = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
         _check(lib().hmpc_solve_device(self._h, d_records.data_ptr(), B, d_wrench.data_ptr(), d_status.data_ptr(),
                                        ctypes.c_void_p(st)))
+
+    def solve_device_warm(self, d_records, B: int, d_wrench, d_status, d_tau=None, d_shift=None, stream=None) -> None:
+        """solve_device warm-started from each robot's working set of its last warm call (hmpc_solve_device_warm).
+        `d_tau` f32 [B,10] or None; `d_shift` i32 [B] on the GPU or None (every robot moved one step)."""
+        import torch
+
+        st = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        _check(lib().hmpc_solve_device_warm(self._h, d_records.data_ptr(), B, d_wrench.data_ptr(), d_status.data_ptr(),
+                                            d_tau.data_ptr() if d_tau is not None else None,
+                                            d_shift.data_ptr() if d_shift is not None else None, ctypes.c_void_p(st)))
 
     def assemble_device(self, d_records, B: int, stream=None) -> dict:
         """Parity hook: un-reduced fp32 QP data of B packed records (torch tensors on the GPU)."""

@@ -237,6 +237,26 @@ struct hmpc_rollout_t
  * the context; hmpc_reset_warm_start forgets them (a new loop on the same context).  HMPC_WARM_START=0 in the environment
  * at hmpc_create keeps every tick a cold start. */
 HMPC_EXTERNC int hmpc_reset_warm_start(hmpc_ctx* ctx, void* stream);
+
+/* Warm start in the caller's own loop (a batched simulator, an RL environment, a host program).  The same working-set memory
+ * as the rollout: slot i belongs to robot i of the batch, every warm call records each robot's optimal working set there and
+ * proposes it to that robot's next warm call.  shift[i] = MPC steps robot i's horizon moved since its last warm call on this
+ * context: NULL = every robot 1 (one call per MPC tick), 0 = the same horizon again, < 0 = no history (e.g. an environment
+ * reset: a cold solve whose working set is still recorded).  The optimum is the same point as a cold solve's; bits 8..19 of
+ * the status count changes relative to the proposal.  The proposal feeds the block start of the active-set stage, which
+ * runs for working-set capacities of up to 31 rows: horizons up to 13 in the single-support class, up to 10 in the
+ * double-support class.  Beyond that a warm call is a cold solve, bit for bit.  HMPC_WARM_START=0 at hmpc_create makes
+ * every warm call a cold solve.
+ *   hmpc_solve_device_warm: as hmpc_solve_device_ex; d_shift NULL or device int [B].  Same argument checks.
+ *   hmpc_solve_batch_warm : as hmpc_solve_batch_ex (all three host-buffer modes); shift NULL or host int [B]. */
+HMPC_EXTERNC int hmpc_solve_device_warm(hmpc_ctx* ctx, const void* d_records, int B, float* d_wrench, int* d_status,
+                                        float* d_tau, const int* d_shift, void* stream);
+HMPC_EXTERNC int hmpc_solve_batch_warm(hmpc_ctx* ctx, const struct update_data_t* in, int B, double* wrench_out,
+                                       double* tau_out, int* status, const int* shift);
+/* The reference boundary warm-started: after hmpc_reference_set_warm_start(1), every update_problem_data proposes the
+ * previous call's working set moved one step (a hmpc_solve_batch_warm with shift NULL on the one-robot context).
+ * setup_problem with another dt, f_max or horizon forgets it.  Default 0: every tick a cold start, like the reference. */
+HMPC_EXTERNC void hmpc_reference_set_warm_start(int on);
 /* ticks >= 1.  d_wrench_log: NULL or float [ticks][B][12] (first-step wrench of every tick); d_record_log: NULL or
  * [ticks][B][hmpc_record_bytes] (the packed records the solver saw, for after-the-fact parity checks). */
 HMPC_EXTERNC int hmpc_rollout_device(hmpc_ctx* ctx, struct hmpc_state_t* d_states, struct hmpc_rollout_t* d_loop, int B,
