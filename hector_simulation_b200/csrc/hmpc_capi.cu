@@ -134,8 +134,9 @@ struct hmpc_ctx {
   int* d_status = nullptr;         // scratch status (assembly hook)
   int* d_counts = nullptr;         // [NCHUNK][2] class list lengths
   int* d_lists = nullptr;          // [NCHUNK][2][max_batch] class lists (host-built, host-buffer path)
-  int* d_cls = nullptr;            // [NCHUNK][2 parities x 4 lengths | class-1 list | class-2 list] (device-resident path)
-  unsigned tick[NCHUNK] = {0, 0, 0, 0};  // calls per slot: parity of the list lengths in use
+  int* d_cls = nullptr;            // [NCHUNK][2 parities x 4 lengths | class-1 list | class-2 list] (device-resident path;
+                                   // slot 0: eager chains, slot 1: chains recorded into a CUDA graph)
+  unsigned tick[NCHUNK] = {0, 0, 0, 0};  // eager calls per slot: parity of the list lengths in use
   unsigned char* h_rec = nullptr;  // pinned
   unsigned char* h_out = nullptr;  // pinned mirror of d_out
   unsigned char* d_states = nullptr;  // hmpc_state_t staging of hmpc_solve_batch_states (row f-1)
@@ -624,6 +625,9 @@ HMPC_EXTERNC int hmpc_set_problem(hmpc_ctx* c, const problem_setup* s)
 
 namespace {
 long long* g_dbg_clk = nullptr;  // profiling hook (hmpc_debug_set_clock_buffer)
+// The slot of d_cls whose list lengths a chain recorded into a CUDA graph uses.  Eager chains use slot 0.
+constexpr int CAPTURE_SLOT = 1;
+static_assert(CAPTURE_SLOT < NCHUNK, "d_cls holds NCHUNK slots");
 // classification pre-pass + one launch per class, all enqueued on `st`
 int enqueue_solve(hmpc_ctx* c, const void* d_records, int B, float* d_wrench32, double* d_wrench64, int* d_status,
                   cudaStream_t st, int slot = 0, float* d_tau = nullptr, int* d_ws = nullptr, int ws_shift = 0, bool ws_read = false,
@@ -633,8 +637,17 @@ int enqueue_solve(hmpc_ctx* c, const void* d_records, int B, float* d_wrench32, 
   CK(cudaSetDevice(c->device));
   // per slot: [2 parities][4 list lengths], then the lists of class 1 and class 2.  No classification kernel: the
   // class-0 launch runs over every instance and hands the ones with more stance blocks than it holds to class 1's list.
+  // An eager chain uses the parity of its call count: the previous call's class-0 launch zeroed those lengths.  A graph
+  // replays the lengths it was recorded with and nothing zeroes them between replays, so a chain recorded into a graph
+  // uses the capture slot, starts with a memset node that zeroes both parities (the wave-barrier counter included), and
+  // leaves the eager call count alone.
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  CK(cudaStreamIsCapturing(st, &cap));
+  const bool capturing = cap != cudaStreamCaptureStatusNone;
+  if (capturing) slot = CAPTURE_SLOT;
   int* base = c->d_cls + (size_t)slot * (8 + 2 * (size_t)c->max_batch);
-  const int par = (c->tick[slot]++) & 1;
+  const int par = capturing ? 0 : (c->tick[slot]++) & 1;
+  if (capturing) CK(cudaMemsetAsync(base, 0, 8 * sizeof(int), st));
   int* counts = base + 4 * par;
   int* counts_next = base + 4 * (par ^ 1);
   int* lists = base + 8 - (size_t)c->max_batch;  // lists + i * max_batch is class i's list, i = 1, 2

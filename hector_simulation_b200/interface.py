@@ -334,7 +334,8 @@ class BatchedMPC:
         return (wrench, tau, status) if torques else (wrench, status)
 
     def prepare_device(self, d_states, B: int, d_records, stream=None, dt_mpc: float = 0.04) -> None:
-        """Row f-1 on device-resident data: torch uint8 [B,352] states -> packed records [B,stride]."""
+        """Row f-1 on device-resident data: torch uint8 [B,352] states -> packed records [B,stride].
+        Capturable in a CUDA graph (torch.cuda.graph; include/hector_mpc_b200.h, "CUDA graphs")."""
         import torch
 
         st = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
@@ -343,7 +344,8 @@ class BatchedMPC:
     def rollout_device(self, d_states, d_loop, B: int, ticks: int, d_wrench_log=None, d_record_log=None, stream=None,
                        dt_mpc: float = 0.04) -> None:
         """Row f-3: `ticks` closed-loop ticks (prepare -> solve -> advance) enqueued on one stream, no host in the
-        loop.  torch CUDA tensors: states uint8 [B,352], loop uint8 [B,80], logs f32 [ticks,B,12] / uint8 [ticks,B,stride]."""
+        loop.  torch CUDA tensors: states uint8 [B,352], loop uint8 [B,80], logs f32 [ticks,B,12] / uint8 [ticks,B,stride].
+        Capturable in a CUDA graph: every replay advances the states and the loop by `ticks` ticks."""
         import torch
 
         st = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
@@ -375,7 +377,8 @@ class BatchedMPC:
         _check(lib().hmpc_shard_wait(self._h))
 
     def reset_warm_start(self, stream=None) -> None:
-        """Forget the working sets the closed loop keeps between ticks (a new loop on this context starts cold)."""
+        """Forget the working sets the closed loop keeps between ticks (a new loop on this context starts cold).
+        Capturable in a CUDA graph: every replay clears them."""
         import torch
 
         st = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
@@ -384,7 +387,8 @@ class BatchedMPC:
     def swing_device(self, d_states, d_loop, d_phase, d_swing, B: int, d_cmd, dt: float = 0.001, dt_swing: float = 0.04,
                      stream=None) -> None:
         """Row f-4: one swingLegController::updateSwingLeg per robot on the device.  torch CUDA tensors: states uint8
-        [B,352], loop uint8 [B,80], phase f64 [B], swing uint8 [B,72] (updated in place), cmd uint8 [B,232]."""
+        [B,352], loop uint8 [B,80], phase f64 [B], swing uint8 [B,72] (updated in place), cmd uint8 [B,232].
+        Capturable in a CUDA graph: every replay updates `d_swing`."""
         import torch
 
         st = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
@@ -392,7 +396,8 @@ class BatchedMPC:
                                        B, dt, dt_swing, d_cmd.data_ptr(), ctypes.c_void_p(st)))
 
     def solve_device(self, d_records, B: int, d_wrench, d_status, stream=None) -> None:
-        """Device-resident path.  Arguments are torch CUDA tensors (uint8 [B,stride], f32 [B,12N], i32 [B])."""
+        """Device-resident path.  Arguments are torch CUDA tensors (uint8 [B,stride], f32 [B,12N], i32 [B]).
+        Capturable in a CUDA graph: a replay solves what the captured tensors hold at that time."""
         import torch
 
         st = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
@@ -401,7 +406,8 @@ class BatchedMPC:
 
     def solve_device_warm(self, d_records, B: int, d_wrench, d_status, d_tau=None, d_shift=None, stream=None) -> None:
         """solve_device warm-started from each robot's working set of its last warm call (hmpc_solve_device_warm).
-        `d_tau` f32 [B,10] or None; `d_shift` i32 [B] on the GPU or None (every robot moved one step)."""
+        `d_tau` f32 [B,10] or None; `d_shift` i32 [B] on the GPU or None (every robot moved one step).
+        Capturable in a CUDA graph: every replay proposes and records working sets, reading `d_shift` when it runs."""
         import torch
 
         st = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream

@@ -311,6 +311,22 @@ HMPC_EXTERNC int hmpc_swing_device(hmpc_ctx* ctx, const struct hmpc_state_t* d_s
                                    const double* d_phase, struct hmpc_swing_t* d_swing, int B, double dt, double dtSwing,
                                    struct hmpc_swing_cmd_t* d_cmd, void* stream);
 
+/* CUDA graphs.  The device-resident calls can be recorded into a CUDA graph by stream capture (cudaStreamBeginCapture,
+ * torch.cuda.graph, ...) on the stream they are given: hmpc_solve_device, hmpc_solve_device_ex, hmpc_solve_device_warm,
+ * hmpc_prepare_device, hmpc_rollout_device, hmpc_swing_device and hmpc_reset_warm_start.  Each launch of the graph gives
+ * the results an eager call on the same inputs gives, bit for bit.
+ *   - A replay is a real call.  A captured warm solve proposes and records working sets, a captured rollout advances
+ *     d_states and d_loop, a captured hmpc_reset_warm_start clears the working sets, every time the graph is launched.
+ *   - A context's calls, eager ones and graph launches alike, must be ordered on one stream (or by events).  All chains
+ *     a context records share one set of class lists, so two graphs of one context, or one graph launched twice, must not
+ *     run concurrently.
+ *   - The pointers and B are frozen into the graph: to solve other inputs, write them into the captured buffers.
+ *   - A graph must not be launched after hmpc_destroy of its context.
+ *   - A call that returns an error while its stream is capturing may have recorded part of its work: end the capture
+ *     and discard the graph.  Argument errors are found before anything is enqueued.
+ * The host-buffer calls (hmpc_solve_batch, _ex, _warm, _states, hmpc_solve_batch_sharded) and the reference boundary
+ * (update_problem_data) wait for their own streams and cannot be captured. */
+
 /* number of kernel launches hmpc_solve_device enqueues per call (classification pre-pass + one per size class) */
 HMPC_EXTERNC int hmpc_launches_per_solve(const hmpc_ctx* ctx);
 /* launch configuration of size class `cls` (0 or 1): out[0..5] = threads per CTA, dynamic shared memory bytes,
