@@ -129,12 +129,19 @@ struct hmpc_ctx {
   problem_setup setup{};
   ClassCfg cls[3];
   int ncls = 0;
+  // refinement class (hmpc_set_refinement): instances beyond the conditioning limit are solved again with iterative
+  // refinement against the stored Hessian instead of ending with code 4
+  ClassCfg ref{};
+  int refine = 0;
+  double kappa_refine = 1.5e4;   // hand-over threshold of classes 0-2 while refinement is on (HMPC_KAPPA_REFINE; DESIGN.md §2)
+  double kappa_max_refined = 1e9;  // conditioning limit of the refinement class (HMPC_KAPPA_MAX_REFINED)
+  int* d_ref = nullptr;            // host-buffer path: [NCHUNK][1 + max_batch] refinement list length + list
   unsigned char* d_rec = nullptr;
   unsigned char* d_out = nullptr;  // host-buffer path: per chunk [wrench floats | status ints], contiguous
   int* d_status = nullptr;         // scratch status (assembly hook)
   int* d_counts = nullptr;         // [NCHUNK][2] class list lengths
   int* d_lists = nullptr;          // [NCHUNK][2][max_batch] class lists (host-built, host-buffer path)
-  int* d_cls = nullptr;            // [NCHUNK][2 parities x 4 lengths | class-1 list | class-2 list] (device-resident path;
+  int* d_cls = nullptr;            // [NCHUNK][2 parities x 8 words | class-1 list | class-2 list | refinement list] (device-resident path;
                                    // slot 0: eager chains, slot 1: chains recorded into a CUDA graph)
   unsigned tick[NCHUNK] = {0, 0, 0, 0};  // eager calls per slot: parity of the list lengths in use
   unsigned char* h_rec = nullptr;  // pinned
@@ -184,10 +191,16 @@ namespace {
 //   0/1: horizon 10 fixed at compile time (class 0: 4 warps, 6 CTAs/SM — shared memory would allow 7, but at 7 the
 //        register budget of 72 spills more and the 1024-robot batch was slower on the H100; class 1: 8 warps)
 //   10 + 5*cls + b: runtime horizon, b-th entry of {64, 128, 192, 256, 384} threads
+//   20 + b: the refinement class, b-th entry of the same (one CTA per SM: it is rare and its shared memory is large)
 #define HMPC_FOR_VARIANT(V, X)                   \
   switch (V) {                                   \
     case 0: X(128, 6, 10, 0); break;             \
     case 1: X(256, 2, 10, 1); break;             \
+    case 20: X(64, 1, 0, 3); break;              \
+    case 21: X(128, 1, 0, 3); break;             \
+    case 22: X(192, 1, 0, 3); break;             \
+    case 23: X(256, 1, 0, 3); break;             \
+    case 24: X(384, 1, 0, 3); break;             \
     case 10: X(64, 8, 0, 0); break;              \
     case 11: X(128, 6, 0, 0); break;             \
     case 12: X(192, 3, 0, 0); break;             \
@@ -312,6 +325,74 @@ int build_classes(hmpc_ctx* c)
   return HMPC_OK;
 }
 
+// The refinement class (hmpc_set_refinement): class 2's shape — no column cache, as many working-set slots as shared memory
+// holds — plus the float32 H tiles and g that its refinement rounds read (refine_layout).  It holds double support (2N
+// blocks) while that leaves at least class 1's working-set capacity, i.e. up to horizon 14; beyond that single support
+// (N blocks), and an instance with more stance blocks keeps its code 4.
+int build_refine_class(hmpc_ctx* c)
+{
+  const int N = c->horizon;
+  ClassCfg& k = c->ref;
+  for (int nb = 2 * N;; nb = N) {
+    const int n = 6 * nb, nt8 = (n + 7) / 8;
+    const int w_sweep = (nt8 + 1) / 2, w_rows = (nb + 2) / 3, warps = w_sweep > w_rows ? w_sweep : w_rows;
+    int bucket = 0;
+    while (bucket < 4 && kBucketThreads[bucket] < 32 * warps) bucket++;
+    k.nb_cap = k.nb_hi = nb;
+    k.variant = 20 + bucket;
+    k.threads = kBucketThreads[bucket];
+    k.tcap = 0;
+    k.qmax = n;
+    k.L = hmpc::refine_layout(N, nb, k.qmax, c->rec_stride, k.threads / 32);
+    while (k.L.total > 226 * 1024 && k.qmax > 4) {
+      k.qmax -= 4;
+      k.L = hmpc::refine_layout(N, nb, k.qmax, c->rec_stride, k.threads / 32);
+    }
+    if (nb == N || (k.L.total <= 226 * 1024 && k.qmax >= hmpc::class_qmax(N, 1))) break;
+  }
+  k.smem = k.L.total;
+  int occ = 0;
+  if (cuda_fail(prep_class(k, &occ), "kernel attribute/occupancy (refinement class)")) return HMPC_ERR_CUDA;
+  if (occ < 1) { g_err = "refinement-class kernel does not fit on this device"; return HMPC_ERR_CUDA; }
+  k.grid_cap = occ * c->sm_count;
+  return HMPC_OK;
+}
+
+// the hand-over threshold of classes 0-2: the refinement threshold while refinement is on, else the conditioning limit
+double kappa_handover(const hmpc_ctx* c) { return c->refine ? c->kappa_refine : c->kappa_max; }
+
+// arguments of a refinement-class launch over `list` (length at *count, device memory)
+hmpc::KernelArgs refine_args(const hmpc_ctx* c, const void* d_records, const update_data_t* raw, int B, float* d_wrench32,
+                             double* d_wrench64, int* d_status, float* d_tau, int* d_ws, const int* list, int* count)
+{
+  const ClassCfg& k = c->ref;
+  hmpc::KernelArgs ka{};
+  ka.records = static_cast<const unsigned char*>(d_records);
+  ka.raw_records = reinterpret_cast<const unsigned char*>(raw);
+  ka.rec_stride = c->rec_stride;
+  ka.batch = B;
+  ka.horizon = c->horizon;
+  ka.dt = c->setup.dt;
+  ka.f_max = c->setup.f_max;
+  ka.max_iter = c->max_iter;
+  ka.tol_kkt = 1e-9;
+  ka.tol_dep = 1e-11;
+  ka.kappa_max = c->kappa_max_refined;
+  ka.wrench = d_wrench32;
+  ka.wrench64 = d_wrench64;
+  ka.status = d_status;
+  ka.tau = d_tau;
+  ka.ws_state = d_ws;  // warm_start 0: no proposal; the class records an empty set
+  ka.list = list;
+  ka.counts = count;   // counts[cls] with cls 0
+  ka.split_nb = -1;
+  ka.nb_cap = k.nb_cap;
+  ka.qmax = k.qmax;
+  ka.tcap = 0;
+  ka.L = k.L;
+  return ka;
+}
+
 hmpc::KernelArgs base_args(const hmpc_ctx* c, const void* d_records, int B, float* d_wrench, int* d_status)
 {
   hmpc::KernelArgs ka{};
@@ -326,7 +407,7 @@ hmpc::KernelArgs base_args(const hmpc_ctx* c, const void* d_records, int B, floa
   ka.tol_dep = 1e-11;
   ka.block_rounds = c->block_rounds;
   ka.block_min = c->block_min;
-  ka.kappa_max = c->kappa_max;
+  ka.kappa_max = kappa_handover(c);
   ka.wrench = d_wrench;
   ka.status = d_status;
   return ka;
@@ -520,6 +601,7 @@ HMPC_EXTERNC void hmpc_destroy(hmpc_ctx* c)
   if (c->d_counts) cudaFree(c->d_counts);
   if (c->d_lists) cudaFree(c->d_lists);
   if (c->d_cls) cudaFree(c->d_cls);
+  if (c->d_ref) cudaFree(c->d_ref);
   shard_release(c);
   if (c->d_ws) cudaFree(c->d_ws);
   if (c->d_shift) cudaFree(c->d_shift);
@@ -579,21 +661,24 @@ HMPC_EXTERNC hmpc_ctx* hmpc_create(int max_batch, int horizon, int device)
           cuda_fail(cudaMemset(c->d_ws, 0, (size_t)max_batch * hmpc::WS_STATE_INTS * sizeof(int)), "cudaMemset working sets") ||
           cuda_fail(cudaMalloc(&c->d_shift, (size_t)max_batch * sizeof(int)), "cudaMalloc shifts") ||
           cuda_fail(cudaMallocHost(&c->h_shift, (size_t)max_batch * sizeof(int)), "cudaMallocHost shifts") ||
-          cuda_fail(cudaMalloc(&c->d_cls, (size_t)NCHUNK * (8 + 2 * (size_t)max_batch) * sizeof(int)), "cudaMalloc class lists") ||
-          cuda_fail(cudaMemset(c->d_cls, 0, (size_t)NCHUNK * (8 + 2 * (size_t)max_batch) * sizeof(int)), "cudaMemset class lists") ||
+          cuda_fail(cudaMalloc(&c->d_cls, (size_t)NCHUNK * (16 + 3 * (size_t)max_batch) * sizeof(int)), "cudaMalloc class lists") ||
+          cuda_fail(cudaMemset(c->d_cls, 0, (size_t)NCHUNK * (16 + 3 * (size_t)max_batch) * sizeof(int)), "cudaMemset class lists") ||
+          cuda_fail(cudaMalloc(&c->d_ref, (size_t)NCHUNK * (1 + (size_t)max_batch) * sizeof(int)), "cudaMalloc refinement lists") ||
           cuda_fail(cudaMalloc(&c->d_status, (size_t)max_batch * 4), "cudaMalloc status") ||
           cuda_fail(cudaMalloc(&c->d_states, (size_t)max_batch * sizeof(hmpc_state_t)), "cudaMalloc states") ||
           cuda_fail(cudaMallocHost(&c->h_states, (size_t)max_batch * sizeof(hmpc_state_t)), "cudaMallocHost states") ||
           cuda_fail(cudaMallocHost(&c->h_rec, (size_t)max_batch * c->rec_stride), "cudaMallocHost records") ||
           cuda_fail(cudaMallocHost(&c->h_out, (size_t)max_batch * (nw * 4 + 4 + 40)), "cudaMallocHost results") ||
           cuda_fail(cudaMallocHost(&c->h_cls, (size_t)NCHUNK * (4 + 3 * (size_t)max_batch) * sizeof(int)), "cudaMallocHost lists") ||
-          build_classes(c) != HMPC_OK;
+          build_classes(c) != HMPC_OK || build_refine_class(c) != HMPC_OK;
   }
   if (!bad) {
     const char* br = getenv("HMPC_BLOCK_ROUNDS");
     if (br) c->block_rounds = atoi(br);
     if (const char* bm = getenv("HMPC_BLOCK_MIN")) c->block_min = atoi(bm);
     if (const char* km = getenv("HMPC_KAPPA_MAX")) c->kappa_max = atof(km);
+    if (const char* kr = getenv("HMPC_KAPPA_REFINE")) c->kappa_refine = atof(kr);
+    if (const char* kx = getenv("HMPC_KAPPA_MAX_REFINED")) c->kappa_max_refined = atof(kx);
     const char* ls = getenv("HMPC_LOCKSTEP");
     if (ls) c->lockstep = atoi(ls);
     const char* wm = getenv("HMPC_WARM_START");
@@ -635,22 +720,23 @@ int enqueue_solve(hmpc_ctx* c, const void* d_records, int B, float* d_wrench32, 
 {
   if (B > c->max_batch) { g_err = "batch exceeds the context's capacity"; return HMPC_ERR_ARG; }
   CK(cudaSetDevice(c->device));
-  // per slot: [2 parities][4 list lengths], then the lists of class 1 and class 2.  No classification kernel: the
-  // class-0 launch runs over every instance and hands the ones with more stance blocks than it holds to class 1's list.
+  // per slot: [2 parities][8 words: list lengths of classes 0-2, wave-barrier counter, refinement list length, 3 unused],
+  // then the lists of class 1, class 2 and the refinement class.  No classification kernel: the class-0 launch runs over
+  // every instance and hands the ones with more stance blocks than it holds to class 1's list.
   // An eager chain uses the parity of its call count: the previous call's class-0 launch zeroed those lengths.  A graph
   // replays the lengths it was recorded with and nothing zeroes them between replays, so a chain recorded into a graph
-  // uses the capture slot, starts with a memset node that zeroes both parities (the wave-barrier counter included), and
-  // leaves the eager call count alone.
+  // uses the capture slot, starts with a memset node that zeroes both parities (the wave-barrier counter and the
+  // refinement list length included), and leaves the eager call count alone.
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   CK(cudaStreamIsCapturing(st, &cap));
   const bool capturing = cap != cudaStreamCaptureStatusNone;
   if (capturing) slot = CAPTURE_SLOT;
-  int* base = c->d_cls + (size_t)slot * (8 + 2 * (size_t)c->max_batch);
+  int* base = c->d_cls + (size_t)slot * (16 + 3 * (size_t)c->max_batch);
   const int par = capturing ? 0 : (c->tick[slot]++) & 1;
-  if (capturing) CK(cudaMemsetAsync(base, 0, 8 * sizeof(int), st));
-  int* counts = base + 4 * par;
-  int* counts_next = base + 4 * (par ^ 1);
-  int* lists = base + 8 - (size_t)c->max_batch;  // lists + i * max_batch is class i's list, i = 1, 2
+  if (capturing) CK(cudaMemsetAsync(base, 0, 16 * sizeof(int), st));
+  int* counts = base + 8 * par;
+  int* counts_next = base + 8 * (par ^ 1);
+  int* lists = base + 16 - (size_t)c->max_batch;  // lists + i * max_batch is class i's list, i = 1, 2; i = 3: refinement
   const bool pdl = pdl_enabled();
   for (int i = 0; i < c->ncls; i++) {
     const ClassCfg& k = c->cls[i];
@@ -671,6 +757,10 @@ int enqueue_solve(hmpc_ctx* c, const void* d_records, int B, float* d_wrench32, 
     ka.counts = counts;
     ka.cls = i;
     ka.esc_list = (i + 1 < c->ncls) ? lists + (size_t)(i + 1) * c->max_batch : nullptr;
+    if (c->refine) {
+      ka.ref_list = lists + (size_t)3 * c->max_batch;
+      ka.ref_count = counts + 4;
+    }
     ka.nb_cap = k.nb_cap;
     ka.qmax = k.qmax;
     ka.tcap = k.tcap;
@@ -678,6 +768,14 @@ int enqueue_solve(hmpc_ctx* c, const void* d_records, int B, float* d_wrench32, 
     ka.dbg_clk = g_dbg_clk;
     const int grid = B < k.grid_cap ? B : k.grid_cap;
     CK(launch_class(k, ka, grid, st, pdl));
+  }
+  if (c->refine) {
+    // the refinement class at the end of the chain: exits at once when nobody was handed over
+    hmpc::KernelArgs ka = refine_args(c, d_records, raw, B, d_wrench32, d_wrench64, d_status, d_tau, d_ws,
+                                      lists + (size_t)3 * c->max_batch, counts + 4);
+    ka.dbg_clk = g_dbg_clk;
+    const int grid = B < c->ref.grid_cap ? B : c->ref.grid_cap;
+    CK(launch_class(c->ref, ka, grid, st, pdl));
   }
   return HMPC_OK;
 }
@@ -726,6 +824,8 @@ int enqueue_solve_hostlists(hmpc_ctx* c, const void* d_records, int nb, int* h_b
     const size_t ints = (n1 > 0) ? (size_t)4 + c->max_batch + n1 : (size_t)4 + n0;
     CK(cudaMemcpyAsync(d_block, h_block, ints * sizeof(int), cudaMemcpyHostToDevice, st));
   }
+  int* d_ref = c->d_ref + (size_t)slot * (1 + (size_t)c->max_batch);  // refinement list length + list of this chunk
+  if (c->refine) CK(cudaMemsetAsync(d_ref, 0, sizeof(int), st));
   for (int i = 0; i < 2; i++) {
     const int cnt = i == 0 ? n0 : n1;
     if (cnt == 0) continue;
@@ -742,6 +842,10 @@ int enqueue_solve_hostlists(hmpc_ctx* c, const void* d_records, int nb, int* h_b
     ka.counts = d_block;
     ka.cls = i;
     ka.esc_list = nullptr;  // overflow is handled by the caller's retry
+    if (c->refine) {        // so is the refinement class (enqueue_refine_retry)
+      ka.ref_list = d_ref + 1;
+      ka.ref_count = d_ref;
+    }
     ka.split_nb = -1;
     ka.nb_cap = k.nb_cap;
     ka.qmax = k.qmax;
@@ -791,6 +895,11 @@ int enqueue_overflow_retry(hmpc_ctx* c, const void* d_records, int nb, int* h_bl
     ka.counts = d_block;
     ka.cls = i;
     ka.esc_list = (i + 1 < c->ncls) ? d_block + 4 + (i + 1) * mb : nullptr;
+    if (c->refine) {
+      int* d_ref = c->d_ref + (size_t)slot * (1 + mb);
+      ka.ref_list = d_ref + 1;
+      ka.ref_count = d_ref;
+    }
     ka.split_nb = -1;
     ka.nb_cap = k.nb_cap;
     ka.qmax = k.qmax;
@@ -800,6 +909,20 @@ int enqueue_overflow_retry(hmpc_ctx* c, const void* d_records, int nb, int* h_bl
     const int grid = cnt < k.grid_cap ? cnt : k.grid_cap;
     CK(launch_class(k, ka, grid, st));
   }
+  return HMPC_OK;
+}
+
+// Refinement in a host-list launch: the kernels pushed the instances beyond the conditioning limit to the chunk's refinement
+// list (device memory), and the refinement class solves them as it does at the end of the device-resident chain.  Called
+// when refinement is on and a status of the chunk has code 4 (a non-positive pivot is not on the list).
+int enqueue_refine_retry(hmpc_ctx* c, const void* d_records, int nb, float* d_wrench32, int* d_status, cudaStream_t st, int slot,
+                         float* d_tau, int* d_ws)
+{
+  int* d_ref = c->d_ref + (size_t)slot * (1 + (size_t)c->max_batch);
+  hmpc::KernelArgs ka = refine_args(c, d_records, nullptr, nb, d_wrench32, nullptr, d_status, d_tau, d_ws, d_ref + 1, d_ref);
+  ka.dbg_clk = g_dbg_clk;
+  const int grid = nb < c->ref.grid_cap ? nb : c->ref.grid_cap;
+  CK(launch_class(c->ref, ka, grid, st));
   return HMPC_OK;
 }
 }  // namespace
@@ -821,14 +944,21 @@ HMPC_EXTERNC void hmpc_debug_set_clock_buffer(long long* d_buf) { g_dbg_clk = d_
 namespace { int g_fail_next_solves = 0; }
 HMPC_EXTERNC void hmpc_debug_fail_next_solves(int n) { g_fail_next_solves = n; }
 
-HMPC_EXTERNC int hmpc_launches_per_solve(const hmpc_ctx* c) { return c ? c->ncls : 0; }
+HMPC_EXTERNC int hmpc_launches_per_solve(const hmpc_ctx* c) { return c ? c->ncls + (c->refine ? 1 : 0) : 0; }
 
-// launch configuration of class `cls`: out[0..5] = threads, dynamic smem bytes, working-set capacity,
-// resident-grid cap (CTAs), max blocks of 6 variables, sweep strip width
+HMPC_EXTERNC int hmpc_set_refinement(hmpc_ctx* c, int on)
+{
+  if (!c) { g_err = "hmpc_set_refinement: null context"; return HMPC_ERR_ARG; }
+  c->refine = on ? 1 : 0;
+  return HMPC_OK;
+}
+
+// launch configuration of class `cls` (HMPC_REFINEMENT_CLASS: the refinement class): out[0..5] = threads, dynamic smem
+// bytes, working-set capacity, resident-grid cap (CTAs), max blocks of 6 variables, sweep strip width
 HMPC_EXTERNC int hmpc_class_config(const hmpc_ctx* c, int cls, int* out)
 {
-  if (!c || !out || cls < 0 || cls >= c->ncls) return HMPC_ERR_ARG;
-  const ClassCfg& k = c->cls[cls];
+  if (!c || !out || cls < 0 || (cls >= c->ncls && cls != HMPC_REFINEMENT_CLASS)) return HMPC_ERR_ARG;
+  const ClassCfg& k = cls == HMPC_REFINEMENT_CLASS ? c->ref : c->cls[cls];
   out[0] = k.threads; out[1] = k.smem; out[2] = k.qmax; out[3] = k.grid_cap; out[4] = k.nb_cap;
   out[5] = 8;  // sweep tile edge (8x8 mma.m8n8k4.f64 accumulator tiles)
   return HMPC_OK;
@@ -1177,9 +1307,11 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
     const size_t ooff = (size_t)b0 * (nw * 4 + 4 + 40);
     {  // working-set overflow (rare, massively degenerate optima): the overflowed instances escalate (enqueue_overflow_retry)
       const int* hs = reinterpret_cast<const int*>(c->h_out + ooff + (size_t)nb * nw * 4);
-      bool overflow = false;
+      bool overflow = false, not_spd = false;
       for (int i = 0; i < nb; i++) overflow |= (HMPC_STATUS_CODE(hs[i]) == hmpc::ST_WS_CAP);
-      if (overflow) {
+      for (int i = 0; i < nb; i++) not_spd |= (HMPC_STATUS_CODE(hs[i]) == hmpc::ST_NOT_SPD);
+      const bool refine = c->refine && not_spd;  // instances handed to the refinement class (on its device-side list)
+      if (overflow || refine) {
         unsigned char* obase = zc ? c->h_out : c->d_out;
         float* dw = reinterpret_cast<float*>(obase + ooff);
         int* ds = reinterpret_cast<int*>(obase + ooff + (size_t)nb * nw * 4);
@@ -1187,8 +1319,12 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
         const unsigned char* rbase = (zc && !sin) ? c->h_rec : c->d_rec;
         int* hblk = c->h_cls + (size_t)k * (4 + 3 * (size_t)c->max_batch);
         const int* sh_k = hsh ? (zc ? hsh : c->d_shift) + b0 : nullptr;  // where the first pass read them
-        int rc = enqueue_overflow_retry(c, rbase + (size_t)b0 * c->rec_stride, nb, hblk, hs, dw, ds, sts[k], k, dt_,
-                                        ws ? ws + (size_t)b0 * hmpc::WS_STATE_INTS : nullptr, sh_k);
+        int* ws_k = ws ? ws + (size_t)b0 * hmpc::WS_STATE_INTS : nullptr;
+        int rc = overflow ? enqueue_overflow_retry(c, rbase + (size_t)b0 * c->rec_stride, nb, hblk, hs, dw, ds, sts[k], k, dt_,
+                                                   ws_k, sh_k)
+                          : HMPC_OK;
+        if (rc == HMPC_OK && refine)
+          rc = enqueue_refine_retry(c, rbase + (size_t)b0 * c->rec_stride, nb, dw, ds, sts[k], k, dt_, ws_k);
         if (rc != HMPC_OK) return rc;
         if (!zc)
           CK(cudaMemcpyAsync(c->h_out + ooff, c->d_out + ooff, (size_t)nb * (nw * 4 + 4 + (tau_out ? 40 : 0)),
@@ -1248,6 +1384,7 @@ int g_has_solved = 0;
 int g_ref_rc = HMPC_OK;       // result of the last update_problem_data (hmpc_reference_last_rc)
 bool g_ref_failing = false;   // inside an episode of failing ticks (the message is printed once per episode)
 bool g_ref_warm = false;      // hmpc_reference_set_warm_start: update_problem_data proposes the previous tick's working set
+bool g_ref_refine = false;    // hmpc_reference_set_refinement: the one-robot context solves beyond the conditioning limit
 
 [[noreturn]] void die(const char* where)
 {
@@ -1266,6 +1403,7 @@ HMPC_EXTERNC void setup_problem(double dt, int horizon, double mu, double f_max)
     if (g_ctx) hmpc_destroy(g_ctx);
     g_ctx = hmpc_create(1, horizon, 0);  // refuses horizons above HMPC_MAX_HORIZON
     if (!g_ctx) die("setup_problem");
+    hmpc_set_refinement(g_ctx, g_ref_refine ? 1 : 0);
     if (!g_blk) {
       void* mem = nullptr;
       const size_t bytes = (sizeof(RefBlock) + 4095) / 4096 * 4096;
@@ -1293,6 +1431,12 @@ HMPC_EXTERNC void setup_problem(double dt, int horizon, double mu, double f_max)
 }
 
 HMPC_EXTERNC void hmpc_reference_set_warm_start(int on) { g_ref_warm = on != 0; }
+
+HMPC_EXTERNC void hmpc_reference_set_refinement(int on)
+{
+  g_ref_refine = on != 0;
+  if (g_ctx) hmpc_set_refinement(g_ctx, g_ref_refine ? 1 : 0);
+}
 
 HMPC_EXTERNC void update_problem_data(double* p, double* v, double* q, double* w, double* r, double* joint_angles,
                                       double yaw, double* weights, double* state_trajectory, double* Alpha_K,

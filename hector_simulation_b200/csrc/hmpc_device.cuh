@@ -42,6 +42,8 @@ struct Layout {
   int Pb, Ws;
   // assembly view of the union
   int rec, x0f, Acd, Bcd, P, M, dd, fbl, comb;
+  // refinement class only (refine_layout): float32 lower H tiles and gradient, kept for the refinement rounds
+  int Hc, gc;
   int total;
 };
 
@@ -98,6 +100,18 @@ __host__ __device__ constexpr Layout make_layout(int N, int nb_cap, int qmax, in
   return L;
 }
 
+// The refinement class (CLS 3): make_layout without column cache, plus two regions that stage 4 would otherwise overwrite —
+// a copy of the float32 lower H tiles (the sweep inverts them in place) and of the gradient (gq becomes zb).
+__host__ __device__ constexpr Layout refine_layout(int N, int nb_cap, int qmax, int rec_stride, int nwarps)
+{
+  Layout L = make_layout(N, nb_cap, qmax, rec_stride, nwarps, 0);
+  const int n = 6 * nb_cap, nt8 = (n + 7) / 8;
+  L.Hc = L.total;
+  L.gc = L.Hc + align16(nt8 * (nt8 + 1) / 2 * 64 * 4);
+  L.total = align16(L.gc + n * 8);
+  return L;
+}
+
 // packed record stride (include/hector_mpc_b200.h: hmpc_record_bytes)
 __host__ __device__ constexpr int record_stride(int N) { return align16((54 + 12 * N) * 4 + 2 * N); }
 
@@ -147,7 +161,10 @@ struct KernelArgs {
   int cls;                       // class index of this launch
   int* esc_list;                 // next class's list (working-set overflow escalation, size-class hand-over) or nullptr
   int split_nb;                  // >= 0: classify in this launch — an instance with more stance blocks goes to esc_list
-  int* counts_next;              // the next call's list lengths, zeroed by this launch (device-resident chain), or nullptr
+  int* ref_list;                 // refinement class's list: instances whose scaled condition number exceeds kappa_max (no
+                                 // non-positive pivot) are pushed here instead of ending with code 4; or nullptr (refinement off)
+  int* ref_count;                // its length word
+  int* counts_next;              // the next call's list lengths (5 words), zeroed by this launch (device-resident chain), or nullptr
   unsigned* wave_sync;           // arrival counter of the wave barrier of multi-wave launches (zero at launch), or nullptr
   int nb_cap;                    // capacity (blocks of 6 variables) the shared-memory carve is sized for
   int qmax;                      // working-set capacity
@@ -929,7 +946,8 @@ __global__ void hmpc_swing_kernel(const unsigned char* states, const unsigned ch
 // the kernel.  NT threads = NT/32 warps: warp w owns tile rows w and NT8-1-w of the sweep, thread e owns
 // constraint row e in the active-set iterations and thread NT-1-i owns variable i.
 // NF > 0 fixes the horizon at compile time (layout offsets and loop bounds fold), NF == 0 reads it from
-// the arguments; CLS = size class (capacity N or 2N blocks of 6 variables).
+// the arguments; CLS = size class (capacity N or 2N blocks of 6 variables), or 3: the refinement class (runtime layout from
+// refine_layout; it refines the final KKT solution against the stored Hessian, see the end of stage 5).
 // ------------------------------------------------------------------------------------------------
 // Profiling hooks (hmpc_debug_set_clock_buffer): HMPC_STAMP(i) = clock of thread 0 at point i (tests/tools/gpu_check.py).
 // Built with -DHMPC_WARP_STAMPS=<k> instead, lane 0 of EVERY warp stamps the phases of block step k of stage 4
@@ -1009,8 +1027,8 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
   uint32_t phase = 0;
   pdl_wait();     // counts / lists / records come from the kernels before this one
   // the list lengths of the NEXT call (the other parity) are cleared here: every kernel of the previous call, which
-  // used them, completed before pdl_wait() returned, and this call only touches its own
-  if (ka.counts_next && blockIdx.x == 0 && tid < 4) ka.counts_next[tid] = 0;
+  // used them, completed before pdl_wait() returned, and this call only touches its own (word 4: the refinement class's)
+  if (ka.counts_next && blockIdx.x == 0 && tid < 5) ka.counts_next[tid] = 0;
   const int count = ka.list ? ka.counts[ka.cls] : ka.batch;
 
   // Batches of more than two waves: the resident CTAs start every wave together (a bounded global barrier between
@@ -1147,6 +1165,12 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
     }
     __syncthreads();
     const int NB = flags[0];
+    if constexpr (CLS == 3) {
+      if (NB > nb_cap) {  // more stance blocks than the refinement class holds: the handing class's code 4 stands
+        __syncthreads();
+        continue;
+      }
+    }
     if (ka.split_nb >= 0 && NB > ka.split_nb) {
       // size classification folded into the launch: more stance blocks than this class holds -> next class's list
       if (tid == 0) {
@@ -1399,6 +1423,13 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
       }
       __syncthreads();
       continue;
+    }
+    if constexpr (CLS == 3) {
+      // the exact QP data for the residuals of the refinement rounds: stage 4 inverts the tiles in place, gq becomes zb
+      float* Hc = reinterpret_cast<float*>(smem + L.Hc);
+      double* gc = reinterpret_cast<double*>(smem + L.gc);
+      for (int e = tid; e < tri(NT8) * 64; e += NT) Hc[e] = Hf[e];
+      for (int e = tid; e < n; e += NT) gc[e] = gq[e];
     }
 
     HMPC_STAMP(3);
@@ -2151,15 +2182,131 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
 
     // working set for the next tick (closed loop): (step, leg) and normal index of every active row.  An instance that
     // overflowed this class's capacity is solved again (by the next class, or the host path's retry) from the same
-    // proposal: it keeps the one it has.
+    // proposal: it keeps the one it has.  The refinement class records an empty set: the next tick starts cold.
     if (ka.ws_state && wid == 0 && code != ST_WS_CAP) {
       int* ws = ka.ws_state + (size_t)inst * WS_STATE_INTS;
-      const unsigned am = (code == ST_OK && qmax <= 31) ? amask[0] : 0u;
+      const unsigned am = (code == ST_OK && qmax <= 31 && CLS != 3) ? amask[0] : 0u;
       if ((am >> lane) & 1u) {
         const int w = wsl[lane];
         ws[1 + __popc(am & ((1u << lane) - 1u))] = (blk_sl[w >> 8] << 8) | (w & 0xff);
       }
       if (lane == 0) ws[0] = __popc(am);
+    }
+
+    bool refined = false;
+    if constexpr (CLS == 3) {
+      // ---------------- refinement class: iterative refinement of the KKT solution against the stored Hessian ----------------
+      // For a badly conditioned H the approximate operators of stages 4-5 (the sweep's H^-1, the explicit S^-1, x
+      // recomposed from the multipliers) leave the optimum visibly off (DESIGN.md §2).  The float32 H and g are the QP's
+      // exact data, so on the final working set W the KKT system  H x - A_W' lam = -g,  A_W x = d_W  is solved again by
+      // iterative refinement: residuals in fp64 against the stored data, r_x = -(Hx + g - A_W' lam), r_lam = d_W - A_W x;
+      // corrections through the same operators (range space): dlam = S^-1 (r_lam - A_W H^-1 r_x), dx = H^-1 (r_x + A_W' dlam).
+      // At most four rounds; converged when a correction moves no component of x by more than the KKT tolerance.  The
+      // answer is then accepted only at a KKT point: every multiplier >= -tol, every row feasible within tol.  Otherwise
+      // (no convergence, or W itself is wrong) the instance keeps code 4.
+      const float* Hc = reinterpret_cast<const float*>(smem + L.Hc);
+      const double* gc = reinterpret_cast<const double*>(smem + L.gc);
+      double* xr = x0;  // refined x (the unconstrained minimiser is spent)
+      double* ub = gq;  // r_x, then r_x + A_W' dlam; zero-padded to whole tiles since stage 2 (zb, which shares it, moves to xr)
+      double* yb = T;   // H^-1 r_x (the class has no column cache: T is one spare column of n)
+      if (code == ST_OK) {
+        if (isvar) xr[vi] = zb[vi];
+        __syncthreads();
+        bool conv = false, contracting = false;
+        double dlast = 1e300;
+        for (int round = 0; round < 4 && !conv; round++) {
+          double rx = 0.0;
+          if (isvar) {
+            // row vi of the stored H (lower tiles, diagonal tiles complete) times x; A_W' lam restricted to the row's block
+            const int I = vi >> 3, ir = vi & 7;
+            double hx = 0.0;
+            for (int j = 0; j < n; j++) {
+              const int J = j >> 3;
+              const float h = (J <= I) ? Hc[toff(I, J) + ir * 8 + (j & 7)] : Hc[toff(J, I) + (j & 7) * 8 + ir];
+              hx = fma((double)h, xr[j], hx);
+            }
+            const int kb = vi / 6, c = vi - 6 * kb;
+            double atl = 0.0;
+            for (int j = 0; j < qhf; j++) {
+              const int w = wsl[j];
+              if (((amask[j >> 5] >> (j & 31)) & 1u) && (w >> 8) == kb) atl = fma(lam[j], nrm[(w & 0xff) * 6 + c], atl);
+            }
+            rx = DS(DS(atl, hx), gc[vi]);
+            ub[vi] = rx;
+          }
+          if (wid == 0) {
+            for (int s2 = lane; s2 < qhf; s2 += 32) {
+              double acc = 0.0;
+              if ((amask[s2 >> 5] >> (s2 & 31)) & 1u) {
+                const int w = wsl[s2], ki = w >> 8, te = (w & 0xff) % 10;
+                acc = ((te == 5) ? -(double)0.01f : ((te == 9) ? -fz[ki] : 0.0)) - dot6(nrm + (w & 0xff) * 6, xr + 6 * ki);
+              }
+              dvs[s2] = acc;  // r_lam
+            }
+          }
+          __syncthreads();
+          if (isvar) yb[vi] = hinv_rowdot(Hd, vi, NT8, ub);
+          __syncthreads();
+          if (wid == 0) {
+            for (int s2 = lane; s2 < qhf; s2 += 32) {
+              double acc = 0.0;
+              if ((amask[s2 >> 5] >> (s2 & 31)) & 1u) {
+                const int w = wsl[s2];
+                acc = dvs[s2] - dot6(nrm + (w & 0xff) * 6, yb + 6 * (w >> 8));
+              }
+              rr[s2] = acc;  // r_lam - A_W H^-1 r_x
+            }
+            __syncwarp();
+            for (int s2 = lane; s2 < qhf; s2 += 32) {
+              double acc = 0.0;
+              if ((amask[s2 >> 5] >> (s2 & 31)) & 1u) {
+                const int rs = tri(s2);
+                for (int j = 0; j < qhf; j++) acc = fma((j <= s2) ? Sv[rs + j] : Sv[tri(j) + s2], rr[j], acc);
+              }
+              dvs[s2] = acc;  // dlam
+              lam[s2] += acc;
+            }
+          }
+          __syncthreads();
+          if (isvar) {
+            const int kb = vi / 6, c = vi - 6 * kb;
+            double acc = rx;
+            for (int j = 0; j < qhf; j++) {
+              const int w = wsl[j];
+              if (((amask[j >> 5] >> (j & 31)) & 1u) && (w >> 8) == kb) acc = fma(dvs[j], nrm[(w & 0xff) * 6 + c], acc);
+            }
+            ub[vi] = acc;
+          }
+          __syncthreads();
+          double dx = 0.0;
+          if (isvar) {
+            dx = hinv_rowdot(Hd, vi, NT8, ub);
+            xr[vi] += dx;
+          }
+          {  // largest correction of the round (non-negative floats order like their bit patterns)
+            const unsigned km = __reduce_max_sync(0xffffffffu, __float_as_uint((float)fabs(dx)));
+            if (lane == 0) redk[16 + wid] = km;
+          }
+          __syncthreads();
+          unsigned kx = redk[16];
+          for (int w = 1; w < NW; w++) kx = redk[16 + w] > kx ? redk[16 + w] : kx;
+          const double dmax = (double)__uint_as_float(kx);
+          contracting = dmax <= 0.5 * dlast;
+          dlast = dmax;
+          conv = dmax <= tol;
+        }
+        // Accepted: converged, or after four rounds still contracting (each correction at most half the one before) with a
+        // last correction below 1e-6 of the solution's scale — the error left is then smaller than that correction.  The
+        // H^-1 of the sweep is the operator error that limits the rate: on h10_lying it contracts by ~0.08 per round.
+        bool bad = !(conv || (contracting && dlast <= 1e3 * tol));
+        if (iscon) bad |= dot6(ne, xr + 6 * ke) - rhs_e < -tol;
+        if (wid == 0)
+          for (int s2 = lane; s2 < qhf; s2 += 32) bad |= ((amask[s2 >> 5] >> (s2 & 31)) & 1u) && lam[s2] < -tol;
+        refined = !__syncthreads_or((int)bad);
+        if (isvar) zb[vi] = xr[vi];
+        __syncthreads();
+      }
+      if (!refined) code = ST_NOT_SPD;  // not solved by refinement either: reported as today
     }
 
     // ---------------- stage 6: scatter (eliminated variables are exactly 0) ----------------
@@ -2204,7 +2351,13 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
         const int slot = atomicAdd(&ka.counts[ka.cls + 1], 1);
         ka.esc_list[slot] = inst;
       }
-      ka.status[inst] = (code & 0xff) | ((iters & 0xfff) << 8) | ((q & 0xff) << 20);
+      if (code == ST_NOT_SPD && flags[3] == ST_OK && ka.ref_list) {  // beyond the conditioning limit, every pivot positive
+        const int slot = atomicAdd(ka.ref_count, 1);
+        ka.ref_list[slot] = inst;
+      }
+      int sw = (code & 0xff) | ((iters & 0xfff) << 8) | ((q & 0xff) << 20);
+      if constexpr (CLS == 3) sw |= refined ? (1 << 28) : 0;  // HMPC_STATUS_REFINED
+      ka.status[inst] = sw;
     }
     __syncthreads();
   }

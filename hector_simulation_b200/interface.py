@@ -30,7 +30,9 @@ EXPORTS = [
     "hmpc_pin_host_buffer", "hmpc_unpin_host_buffer", "hmpc_swing_device",
     "hmpc_reference_last_status", "hmpc_reference_last_rc",
     "hmpc_solve_device_warm", "hmpc_solve_batch_warm", "hmpc_reference_set_warm_start",
+    "hmpc_set_refinement", "hmpc_reference_set_refinement",
 ]
+REFINEMENT_CLASS = 3  # hmpc_class_config index of the refinement class (HMPC_REFINEMENT_CLASS)
 
 SETUP_DTYPE = np.dtype([("dt", "<f4"), ("mu", "<f4"), ("f_max", "<f4"), ("horizon", "<i4")], align=True)
 
@@ -113,6 +115,10 @@ def lib() -> ctypes.CDLL:
         L.hmpc_solve_batch_warm.restype = ctypes.c_int
         L.hmpc_reference_set_warm_start.argtypes = [ctypes.c_int]
         L.hmpc_reference_set_warm_start.restype = None
+        L.hmpc_set_refinement.argtypes = [ctypes.c_void_p, ctypes.c_int]
+        L.hmpc_set_refinement.restype = ctypes.c_int
+        L.hmpc_reference_set_refinement.argtypes = [ctypes.c_int]
+        L.hmpc_reference_set_refinement.restype = None
         _lib = L
     return _lib
 
@@ -169,6 +175,12 @@ def reference_set_warm_start(on: bool) -> None:
     lib().hmpc_reference_set_warm_start(1 if on else 0)
 
 
+def reference_set_refinement(on: bool) -> None:
+    """update_problem_data solves robots beyond the conditioning limit (e.g. lying on their side) through the refinement
+    class instead of reporting them as not solved (hmpc_reference_set_refinement); off by default."""
+    lib().hmpc_reference_set_refinement(1 if on else 0)
+
+
 # ---------------------------------------------------------------------------------------------------
 # Part 2: batched interface
 # ---------------------------------------------------------------------------------------------------
@@ -211,6 +223,11 @@ def status_nactive(s):
     return (np.asarray(s) >> 20) & 0xFF
 
 
+def status_refined(s):
+    """1 where the refinement class solved the instance (HMPC_STATUS_REFINED, bit 28)."""
+    return (np.asarray(s) >> 28) & 1
+
+
 def page_aligned(shape, dtype) -> np.ndarray:
     """A zeroed array that owns whole memory pages (start aligned, size rounded up): what a control loop should hand to
     BatchedMPC.pin / hmpc_pin_host_buffer — a C caller uses posix_memalign the same way."""
@@ -237,6 +254,12 @@ class BatchedMPC:
         s = np.zeros(1, dtype=SETUP_DTYPE)
         s["dt"], s["mu"], s["f_max"], s["horizon"] = dt, mu, f_max, self.horizon
         _check(lib().hmpc_set_problem(self._h, s.ctypes.data))
+
+    def set_refinement(self, on: bool) -> None:
+        """Solve robots beyond the conditioning limit of the sweep inversion (scaled condition number above 1.5e4, e.g. a
+        robot lying on its side) in the refinement class instead of returning code 4 (hmpc_set_refinement).  Off by
+        default.  A refined instance has code 0 and status_refined() == 1; one the class cannot solve keeps code 4."""
+        _check(lib().hmpc_set_refinement(self._h, 1 if on else 0))
 
     @property
     def launches_per_solve(self) -> int:

@@ -121,10 +121,14 @@ typedef struct hmpc_ctx hmpc_ctx;
  *                                    for a robot lying on its side) — the wrench of such an instance is not trusted)
  *   bits  8..19 : working-set changes performed (comparable to qpOASES nWSR)
  *   bits 20..27 : number of active constraints at the solution
+ *   bit  28     : solved by the refinement class (hmpc_set_refinement; code 0).  Only with refinement on.
+ * With refinement on, an instance whose scaled condition number is above 1.5e4 (and below 1e9), with every pivot positive,
+ * is solved again by the refinement class; it returns code 0 with bit 28 set, or code 4 as above.
  */
 #define HMPC_STATUS_CODE(s) ((s) & 0xff)
 #define HMPC_STATUS_ITERS(s) (((s) >> 8) & 0xfff)
 #define HMPC_STATUS_NACTIVE(s) (((s) >> 20) & 0xff)
+#define HMPC_STATUS_REFINED(s) (((s) >> 28) & 1)
 
 #define HMPC_MAX_HORIZON 16 /* dense fp64 working set of one QP must fit one SM's shared memory */
 
@@ -327,10 +331,25 @@ HMPC_EXTERNC int hmpc_swing_device(hmpc_ctx* ctx, const struct hmpc_state_t* d_s
  * The host-buffer calls (hmpc_solve_batch, _ex, _warm, _states, hmpc_solve_batch_sharded) and the reference boundary
  * (update_problem_data) wait for their own streams and cannot be captured. */
 
-/* number of kernel launches hmpc_solve_device enqueues per call (classification pre-pass + one per size class) */
+/* Robots beyond the conditioning limit (INTEGRATION.md).  The fp64 sweep inversion of the solve is accurate up to a scaled
+ * condition number max_i H_ii (H^-1)_ii of about 1e5; above 1.5e5 an instance returns code 4 with no trusted wrench — a
+ * robot lying on its side (about 3e5) is the common case.  hmpc_set_refinement(ctx, 1) hands every instance above 1.5e4 whose
+ * pivots are all positive to the refinement class, one more launch at the end of the solve: it solves the QP again from
+ * the unconstrained minimiser, then refines the KKT solution of the final working set against the stored Hessian (up to
+ * four rounds, residuals in fp64) and accepts it only at a KKT point (code 0 and HMPC_STATUS_REFINED); otherwise the
+ * instance keeps code 4.  Above 1e9, with a non-positive pivot, or with more stance blocks than the class holds (double
+ * support up to horizon 14, single support up to 16) it keeps code 4 as well.  The class records an empty working set: a
+ * warm call after it starts cold.  Default 0: every call, status word and launch as without this switch.  Applies to every
+ * solve of the context (device-resident, host-buffer, rollout).  hmpc_reference_set_refinement does the same for the
+ * reference boundary's one-robot context. */
+HMPC_EXTERNC int hmpc_set_refinement(hmpc_ctx* ctx, int on);
+HMPC_EXTERNC void hmpc_reference_set_refinement(int on);
+
+/* number of kernel launches hmpc_solve_device enqueues per call (one per size class, + the refinement class when on) */
 HMPC_EXTERNC int hmpc_launches_per_solve(const hmpc_ctx* ctx);
-/* launch configuration of size class `cls` (0 or 1): out[0..5] = threads per CTA, dynamic shared memory bytes,
- * working-set capacity, resident-grid cap (CTAs), max blocks of 6 variables, sweep strip width */
+/* launch configuration of size class `cls` (0, 1, 2, or HMPC_REFINEMENT_CLASS): out[0..5] = threads per CTA, dynamic shared
+ * memory bytes, working-set capacity, resident-grid cap (CTAs), max blocks of 6 variables, sweep strip width */
+#define HMPC_REFINEMENT_CLASS 3
 HMPC_EXTERNC int hmpc_class_config(const hmpc_ctx* ctx, int cls, int* out);
 
 /* Debug/parity hook: run only the assembly stage for B packed device records and write the
