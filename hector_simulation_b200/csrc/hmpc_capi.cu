@@ -117,6 +117,9 @@ class HostPool {
 
 constexpr int NCHUNK = 4;  // the host-buffer path pipelines pack / H2D / solve / D2H over this many chunks
 
+// ints of one slot of hmpc_ctx::d_cls: [2 parities x 8 words | class-1 list | class-2 list | refinement list | class-0 list]
+size_t cls_slot_ints(int max_batch) { return 16 + 4 * (size_t)max_batch; }
+
 struct ClassCfg {
   int nb_hi, nb_cap, qmax, threads, smem, grid_cap, variant, tcap;
   hmpc::Layout L;
@@ -141,8 +144,9 @@ struct hmpc_ctx {
   int* d_status = nullptr;         // scratch status (assembly hook)
   int* d_counts = nullptr;         // [NCHUNK][2] class list lengths
   int* d_lists = nullptr;          // [NCHUNK][2][max_batch] class lists (host-built, host-buffer path)
-  int* d_cls = nullptr;            // [NCHUNK][2 parities x 8 words | class-1 list | class-2 list | refinement list] (device-resident path;
+  int* d_cls = nullptr;            // [NCHUNK][cls_slot_ints] class-list lengths and lists (device-resident path;
                                    // slot 0: eager chains, slot 1: chains recorded into a CUDA graph)
+  unsigned char* h_mask = nullptr; // pinned [max_batch]: the mask of hmpc_solve_batch_masked, read mapped by the in-place mode
   unsigned tick[NCHUNK] = {0, 0, 0, 0};  // eager calls per slot: parity of the list lengths in use
   unsigned char* h_rec = nullptr;  // pinned
   unsigned char* h_out = nullptr;  // pinned mirror of d_out
@@ -606,6 +610,7 @@ HMPC_EXTERNC void hmpc_destroy(hmpc_ctx* c)
   if (c->d_ws) cudaFree(c->d_ws);
   if (c->d_shift) cudaFree(c->d_shift);
   if (c->h_shift) cudaFreeHost(c->h_shift);
+  if (c->h_mask) cudaFreeHost(c->h_mask);
   if (c->d_states) cudaFree(c->d_states);
   if (c->h_states) cudaFreeHost(c->h_states);
   if (c->h_rec) cudaFreeHost(c->h_rec);
@@ -661,8 +666,9 @@ HMPC_EXTERNC hmpc_ctx* hmpc_create(int max_batch, int horizon, int device)
           cuda_fail(cudaMemset(c->d_ws, 0, (size_t)max_batch * hmpc::WS_STATE_INTS * sizeof(int)), "cudaMemset working sets") ||
           cuda_fail(cudaMalloc(&c->d_shift, (size_t)max_batch * sizeof(int)), "cudaMalloc shifts") ||
           cuda_fail(cudaMallocHost(&c->h_shift, (size_t)max_batch * sizeof(int)), "cudaMallocHost shifts") ||
-          cuda_fail(cudaMalloc(&c->d_cls, (size_t)NCHUNK * (16 + 3 * (size_t)max_batch) * sizeof(int)), "cudaMalloc class lists") ||
-          cuda_fail(cudaMemset(c->d_cls, 0, (size_t)NCHUNK * (16 + 3 * (size_t)max_batch) * sizeof(int)), "cudaMemset class lists") ||
+          cuda_fail(cudaMallocHost(&c->h_mask, (size_t)max_batch), "cudaMallocHost mask") ||
+          cuda_fail(cudaMalloc(&c->d_cls, (size_t)NCHUNK * cls_slot_ints(max_batch) * sizeof(int)), "cudaMalloc class lists") ||
+          cuda_fail(cudaMemset(c->d_cls, 0, (size_t)NCHUNK * cls_slot_ints(max_batch) * sizeof(int)), "cudaMemset class lists") ||
           cuda_fail(cudaMalloc(&c->d_ref, (size_t)NCHUNK * (1 + (size_t)max_batch) * sizeof(int)), "cudaMalloc refinement lists") ||
           cuda_fail(cudaMalloc(&c->d_status, (size_t)max_batch * 4), "cudaMalloc status") ||
           cuda_fail(cudaMalloc(&c->d_states, (size_t)max_batch * sizeof(hmpc_state_t)), "cudaMalloc states") ||
@@ -713,16 +719,17 @@ long long* g_dbg_clk = nullptr;  // profiling hook (hmpc_debug_set_clock_buffer)
 // The slot of d_cls whose list lengths a chain recorded into a CUDA graph uses.  Eager chains use slot 0.
 constexpr int CAPTURE_SLOT = 1;
 static_assert(CAPTURE_SLOT < NCHUNK, "d_cls holds NCHUNK slots");
-// classification pre-pass + one launch per class, all enqueued on `st`
+// one launch per class, all enqueued on `st`; with `mask` (device-readable [B]) the selection kernel first
 int enqueue_solve(hmpc_ctx* c, const void* d_records, int B, float* d_wrench32, double* d_wrench64, int* d_status,
                   cudaStream_t st, int slot = 0, float* d_tau = nullptr, int* d_ws = nullptr, int ws_shift = 0, bool ws_read = false,
-                  const update_data_t* raw = nullptr, const int* ws_shifts = nullptr)
+                  const update_data_t* raw = nullptr, const int* ws_shifts = nullptr, const unsigned char* mask = nullptr)
 {
   if (B > c->max_batch) { g_err = "batch exceeds the context's capacity"; return HMPC_ERR_ARG; }
   CK(cudaSetDevice(c->device));
   // per slot: [2 parities][8 words: list lengths of classes 0-2, wave-barrier counter, refinement list length, 3 unused],
-  // then the lists of class 1, class 2 and the refinement class.  No classification kernel: the class-0 launch runs over
-  // every instance and hands the ones with more stance blocks than it holds to class 1's list.
+  // then the lists of class 1, class 2, the refinement class and class 0.  No classification kernel: the class-0 launch
+  // runs over every instance (or, in a masked call, over the list the selection kernel built from the mask) and hands the
+  // ones with more stance blocks than it holds to class 1's list.
   // An eager chain uses the parity of its call count: the previous call's class-0 launch zeroed those lengths.  A graph
   // replays the lengths it was recorded with and nothing zeroes them between replays, so a chain recorded into a graph
   // uses the capture slot, starts with a memset node that zeroes both parities (the wave-barrier counter and the
@@ -731,13 +738,22 @@ int enqueue_solve(hmpc_ctx* c, const void* d_records, int B, float* d_wrench32, 
   CK(cudaStreamIsCapturing(st, &cap));
   const bool capturing = cap != cudaStreamCaptureStatusNone;
   if (capturing) slot = CAPTURE_SLOT;
-  int* base = c->d_cls + (size_t)slot * (16 + 3 * (size_t)c->max_batch);
+  int* base = c->d_cls + (size_t)slot * cls_slot_ints(c->max_batch);
   const int par = capturing ? 0 : (c->tick[slot]++) & 1;
   if (capturing) CK(cudaMemsetAsync(base, 0, 16 * sizeof(int), st));
   int* counts = base + 8 * par;
   int* counts_next = base + 8 * (par ^ 1);
-  int* lists = base + 16 - (size_t)c->max_batch;  // lists + i * max_batch is class i's list, i = 1, 2; i = 3: refinement
+  // lists + i * max_batch is class i's list, i = 1, 2; i = 3: the refinement class's; i = 4: class 0's in a masked call
+  int* lists = base + 16 - (size_t)c->max_batch;
+  int* list0 = mask ? lists + (size_t)4 * c->max_batch : nullptr;
   const bool pdl = pdl_enabled();
+  if (mask) {
+    // counts[0] of this parity was cleared by the previous call's class-0 launch: the kernel waits for it (griddepcontrol.wait)
+    // before its first store, and class 0 reads the list after its own wait
+    CK(launch_chain(hmpc::hmpc_select_kernel<hmpc::SELECT_THREADS>, dim3(1), dim3(hmpc::SELECT_THREADS), 0, st, pdl, mask, B,
+                    list0, counts));
+    CK(cudaGetLastError());
+  }
   for (int i = 0; i < c->ncls; i++) {
     const ClassCfg& k = c->cls[i];
     hmpc::KernelArgs ka = base_args(c, d_records, B, d_wrench32, d_status);
@@ -748,7 +764,7 @@ int enqueue_solve(hmpc_ctx* c, const void* d_records, int B, float* d_wrench32, 
     ka.ws_state = d_ws;
     ka.ws_shift = ws_shift;
     ka.ws_shifts = ws_shifts;
-    ka.list = (i == 0) ? nullptr : lists + (size_t)i * c->max_batch;
+    ka.list = (i == 0) ? list0 : lists + (size_t)i * c->max_batch;
     ka.split_nb = (i == 0) ? k.nb_hi : -1;
     ka.counts_next = (i == 0) ? counts_next : nullptr;
     // arrival counter of class 0's wave barrier: the 4th length slot, which the chain does not use.  (Class 1 runs free:
@@ -783,10 +799,10 @@ int enqueue_solve(hmpc_ctx* c, const void* d_records, int B, float* d_wrench32, 
 // the warm-started device-resident solve: robot i's proposal is its set in the context's d_ws, moved d_shift[i] steps
 // (d_shift NULL: every robot one step, the closed loop's tick); HMPC_WARM_START=0 makes it a cold solve
 int enqueue_solve_warm(hmpc_ctx* c, const void* d_records, int B, float* d_wrench, int* d_status, cudaStream_t st, float* d_tau,
-                       const int* d_shift)
+                       const int* d_shift, const unsigned char* d_mask = nullptr)
 {
   return enqueue_solve(c, d_records, B, d_wrench, nullptr, d_status, st, 0, d_tau, c->warm_start ? c->d_ws : nullptr, 1, true,
-                       nullptr, d_shift);
+                       nullptr, d_shift, d_mask);
 }
 }  // namespace
 
@@ -794,13 +810,16 @@ namespace {
 // Host-buffer path: the host has the contact tables in hand while it packs, so it builds the class lists itself
 // (same rule as hmpc_classify_kernel) and launches only the non-empty classes — no classification kernel, no
 // empty launches.  Working-set overflow cannot escalate here; the caller re-runs such a chunk through enqueue_solve.
-void classify_host(const hmpc_ctx* c, const unsigned char* gait0, size_t gait_stride, int nb, int* blockbuf)
+// `mask` (the chunk's, host) or NULL: only the robots it lists go on the lists.
+void classify_host(const hmpc_ctx* c, const unsigned char* gait0, size_t gait_stride, int nb, int* blockbuf,
+                   const unsigned char* mask = nullptr)
 {
   int* counts = blockbuf;
   int* lists = blockbuf + 4;
   counts[0] = counts[1] = counts[2] = counts[3] = 0;
   const int N = c->horizon;
   for (int i = 0; i < nb; i++) {
+    if (mask && !mask[i]) continue;
     int k = 0;
     for (int e = 0; e < 2 * N; e++) {
       const float ub = c->setup.f_max * (float)gait0[(size_t)i * gait_stride + e];
@@ -863,15 +882,17 @@ int enqueue_solve_hostlists(hmpc_ctx* c, const void* d_records, int nb, int* h_b
 // with escalation from the one to the other.  The rest of the chunk keeps its results and its recorded working sets, and an
 // instance that overflowed kept its proposal (the kernel does not record a set for it), so results, statuses and working
 // sets are those of the device-resident path.  `h_block` holds the chunk's class lists and is reused for the retry's.
+// `mask` (the chunk's, host) or NULL: the status words of robots it does not list are stale and are not looked at.
 int enqueue_overflow_retry(hmpc_ctx* c, const void* d_records, int nb, int* h_block, const int* h_status, float* d_wrench32,
-                           int* d_status, cudaStream_t st, int slot, float* d_tau, int* d_ws, const int* ws_shifts)
+                           int* d_status, cudaStream_t st, int slot, float* d_tau, int* d_ws, const int* ws_shifts,
+                           const unsigned char* mask)
 {
   const size_t mb = c->max_batch;
   std::vector<char> was_cls1(nb, 0);
   for (int j = 0; j < h_block[1]; j++) was_cls1[h_block[4 + mb + j]] = 1;
   int n[3] = {0, 0, 0};
   for (int i = 0; i < nb; i++) {
-    if (HMPC_STATUS_CODE(h_status[i]) != hmpc::ST_WS_CAP) continue;
+    if ((mask && !mask[i]) || HMPC_STATUS_CODE(h_status[i]) != hmpc::ST_WS_CAP) continue;
     const int next = was_cls1[i] ? 2 : 1;
     if (next < c->ncls) h_block[4 + next * mb + n[next]++] = i;  // (class 1 as the last class: its overflow is final)
   }
@@ -991,6 +1012,18 @@ HMPC_EXTERNC int hmpc_solve_device_warm(hmpc_ctx* c, const void* d_records, int 
   return enqueue_solve_warm(c, d_records, B, d_wrench, d_status, static_cast<cudaStream_t>(stream), d_tau, d_shift);
 }
 
+HMPC_EXTERNC int hmpc_solve_device_masked(hmpc_ctx* c, const void* d_records, int B, const unsigned char* d_mask, float* d_wrench,
+                                          int* d_status, float* d_tau, const int* d_shift, void* stream)
+{
+  if (!c || !d_records || !d_mask || !d_wrench || !d_status || B < 0) {
+    g_err = "hmpc_solve_device_masked: bad argument";
+    return HMPC_ERR_ARG;
+  }
+  if (B == 0) return HMPC_OK;
+  if (int rc = check_device_records(c, d_records, B, "hmpc_solve_device_masked")) return rc;
+  return enqueue_solve_warm(c, d_records, B, d_wrench, d_status, static_cast<cudaStream_t>(stream), d_tau, d_shift, d_mask);
+}
+
 HMPC_EXTERNC int hmpc_assemble_device(hmpc_ctx* c, const void* d_records, int B, float* d_H, float* d_g,
                                       float* d_Fblk, float* d_lb, float* d_ub, void* stream)
 {
@@ -1023,7 +1056,8 @@ HMPC_EXTERNC int hmpc_assemble_device(hmpc_ctx* c, const void* d_records, int B,
 }
 
 static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_state_t* sin, int B, double* wrench_out,
-                            double* tau_out, int* status, double dtMPC = 0.0, bool warm = false, const int* shift = nullptr);
+                            double* tau_out, int* status, double dtMPC = 0.0, bool warm = false, const int* shift = nullptr,
+                            const unsigned char* mask = nullptr);
 
 HMPC_EXTERNC int hmpc_solve_batch(hmpc_ctx* c, const update_data_t* in, int B, double* wrench_out, int* status)
 {
@@ -1041,6 +1075,13 @@ HMPC_EXTERNC int hmpc_solve_batch_warm(hmpc_ctx* c, const update_data_t* in, int
 {
   if (!in) { g_err = "hmpc_solve_batch_warm: bad argument (null records)"; return HMPC_ERR_ARG; }
   return solve_batch_impl(c, in, nullptr, B, wrench_out, tau_out, status, 0.0, true, shift);
+}
+
+HMPC_EXTERNC int hmpc_solve_batch_masked(hmpc_ctx* c, const update_data_t* in, int B, const unsigned char* mask, double* wrench_out,
+                                         double* tau_out, int* status, const int* shift)
+{
+  if (!in || !mask) { g_err = "hmpc_solve_batch_masked: bad argument (null records or mask)"; return HMPC_ERR_ARG; }
+  return solve_batch_impl(c, in, nullptr, B, wrench_out, tau_out, status, 0.0, true, shift, mask);
 }
 
 static_assert(sizeof(hmpc_state_t) == 352 && offsetof(hmpc_state_t, gait) == 39 * 8, "hmpc_state_t layout (hmpc_prepare_kernel)");
@@ -1183,14 +1224,22 @@ HMPC_EXTERNC int hmpc_solve_batch_states(hmpc_ctx* c, const hmpc_state_t* in, in
   return solve_batch_impl(c, nullptr, in, B, wrench_out, tau_out, status, dtMPC);
 }
 
+// mask (hmpc_solve_batch_masked) or NULL: only the robots it lists are solved, and only their rows of wrench_out, tau_out and
+// status are written; the context's staging rows of the others keep stale results, which nothing reads
 static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_state_t* sin, int B, double* wrench_out,
-                            double* tau_out, int* status, double dtMPC, bool warm, const int* shift)
+                            double* tau_out, int* status, double dtMPC, bool warm, const int* shift, const unsigned char* mask)
 {
   if (!c || (!in && !sin) || !wrench_out || B < 0 || B > c->max_batch) {
     g_err = "hmpc_solve_batch: bad argument (null pointer or batch > capacity)";
     return HMPC_ERR_ARG;
   }
   if (B == 0) return HMPC_OK;
+  if (mask) {
+    bool any = false;
+    for (int i = 0; i < B && !any; i++) any = mask[i] != 0;
+    if (!any) return HMPC_OK;
+  }
+  auto listed = [mask](int i) { return !mask || mask[i] != 0; };
   if (g_fail_next_solves > 0) {
     g_fail_next_solves--;
     g_err = "injected failure (hmpc_debug_fail_next_solves)";
@@ -1226,7 +1275,9 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
     // the device-resident chain on the caller's records: class 0 classifies on the way, overflow escalates on the device
     int* ds = status ? status : reinterpret_cast<int*>(c->h_out + (size_t)c->max_batch * nw * 4);
     float* dt_ = tau_out ? reinterpret_cast<float*>(c->h_out + (size_t)c->max_batch * (nw * 4 + 4)) : nullptr;
-    int rc = enqueue_solve(c, nullptr, B, c->shard_out, wrench_out, ds, c->stream, 0, dt_, ws, 1, ws != nullptr, in, hsh);
+    if (mask) memcpy(c->h_mask, mask, (size_t)B);  // pinned: the selection kernel reads it mapped
+    int rc = enqueue_solve(c, nullptr, B, c->shard_out, wrench_out, ds, c->stream, 0, dt_, ws, 1, ws != nullptr, in, hsh,
+                           mask ? c->h_mask : nullptr);
     if (rc != HMPC_OK) return rc;
     if (c->shard_out) {
       CK(cudaEventRecord(c->solved, c->stream));
@@ -1234,9 +1285,12 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
     }
     CK(cudaStreamSynchronize(c->stream));
     bool all_ok = true;
-    for (int i = 0; i < B; i++) all_ok &= (HMPC_STATUS_CODE(ds[i]) == 0);
+    for (int i = 0; i < B; i++)
+      if (listed(i)) all_ok &= (HMPC_STATUS_CODE(ds[i]) == 0);
     if (tau_out)
-      for (int i = 0; i < B * 10; i++) tau_out[i] = (double)dt_[i];
+      for (int i = 0; i < B; i++)
+        if (listed(i))
+          for (int j = 0; j < 10; j++) tau_out[(size_t)i * 10 + j] = (double)dt_[(size_t)i * 10 + j];
     if (!all_ok) { g_err = "hmpc_solve_batch: at least one instance did not reach a KKT point (see status[])"; return HMPC_ERR_NOT_CONVERGED; }
     return HMPC_OK;
   }
@@ -1261,13 +1315,20 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
                                c->d_rec + (size_t)b0 * c->rec_stride, sts[k]);
       if (rc != HMPC_OK) return rc;
     } else {
+      // robots [r0, r1): all of them, or only the listed ones (the kernels read no other record)
+      auto pack = [&](int r0, int r1) {
+        if (!mask) return hmpc_pack_records(in + r0, r1 - r0, c->horizon, c->h_rec + (size_t)r0 * c->rec_stride);
+        for (int i = r0; i < r1; i++)
+          if (mask[i]) hmpc_pack_records(in + i, 1, c->horizon, c->h_rec + (size_t)i * c->rec_stride);
+        return (int)HMPC_OK;
+      };
       if (c->pool && nb >= 128) {
         c->pool->parallel([&](int part, int nparts) {
           const int p0 = (int)((long long)nb * part / nparts), p1 = (int)((long long)nb * (part + 1) / nparts);
-          hmpc_pack_records(in + b0 + p0, p1 - p0, c->horizon, c->h_rec + (size_t)(b0 + p0) * c->rec_stride);
+          pack(b0 + p0, b0 + p1);
         });
       } else {
-        rc = hmpc_pack_records(in + b0, nb, c->horizon, c->h_rec + (size_t)b0 * c->rec_stride);
+        rc = pack(b0, b0 + nb);
       }
       if (rc != HMPC_OK) return rc;
       if (trace) tr[ntr++] = now();
@@ -1283,7 +1344,7 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
     const unsigned char* rbase = (zc && !sin) ? c->h_rec : c->d_rec;
     int* hblk = c->h_cls + (size_t)k * (4 + 3 * (size_t)c->max_batch);
     if (sin) classify_host(c, sin[b0].gait, sizeof(hmpc_state_t), nb, hblk);
-    else classify_host(c, in[b0].gait, sizeof(update_data_t), nb, hblk);
+    else classify_host(c, in[b0].gait, sizeof(update_data_t), nb, hblk, mask ? mask + b0 : nullptr);
     int* ws_k = ws ? ws + (size_t)b0 * hmpc::WS_STATE_INTS : nullptr;
     const int* sh_k = nullptr;
     if (hsh && zc) {
@@ -1308,8 +1369,8 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
     {  // working-set overflow (rare, massively degenerate optima): the overflowed instances escalate (enqueue_overflow_retry)
       const int* hs = reinterpret_cast<const int*>(c->h_out + ooff + (size_t)nb * nw * 4);
       bool overflow = false, not_spd = false;
-      for (int i = 0; i < nb; i++) overflow |= (HMPC_STATUS_CODE(hs[i]) == hmpc::ST_WS_CAP);
-      for (int i = 0; i < nb; i++) not_spd |= (HMPC_STATUS_CODE(hs[i]) == hmpc::ST_NOT_SPD);
+      for (int i = 0; i < nb; i++) overflow |= listed(b0 + i) && (HMPC_STATUS_CODE(hs[i]) == hmpc::ST_WS_CAP);
+      for (int i = 0; i < nb; i++) not_spd |= listed(b0 + i) && (HMPC_STATUS_CODE(hs[i]) == hmpc::ST_NOT_SPD);
       const bool refine = c->refine && not_spd;  // instances handed to the refinement class (on its device-side list)
       if (overflow || refine) {
         unsigned char* obase = zc ? c->h_out : c->d_out;
@@ -1321,7 +1382,7 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
         const int* sh_k = hsh ? (zc ? hsh : c->d_shift) + b0 : nullptr;  // where the first pass read them
         int* ws_k = ws ? ws + (size_t)b0 * hmpc::WS_STATE_INTS : nullptr;
         int rc = overflow ? enqueue_overflow_retry(c, rbase + (size_t)b0 * c->rec_stride, nb, hblk, hs, dw, ds, sts[k], k, dt_,
-                                                   ws_k, sh_k)
+                                                   ws_k, sh_k, mask ? mask + b0 : nullptr)
                           : HMPC_OK;
         if (rc == HMPC_OK && refine)
           rc = enqueue_refine_retry(c, rbase + (size_t)b0 * c->rec_stride, nb, dw, ds, sts[k], k, dt_, ws_k);
@@ -1332,13 +1393,23 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
         CK(cudaStreamSynchronize(sts[k]));
       }
     }
-    if (tau_out) {
-      const float* ht = reinterpret_cast<const float*>(c->h_out + ooff + (size_t)nb * (nw * 4 + 4));
-      for (int i = 0; i < nb * 10; i++) tau_out[(size_t)b0 * 10 + i] = (double)ht[i];
-    }
     const float* src = reinterpret_cast<const float*>(c->h_out + ooff);
     const int* hst = reinterpret_cast<const int*>(c->h_out + ooff + (size_t)nb * nw * 4);
     double* dst = wrench_out + (size_t)b0 * nw;
+    const float* ht = reinterpret_cast<const float*>(c->h_out + ooff + (size_t)nb * (nw * 4 + 4));
+    if (mask) {  // the listed rows only
+      for (int i = 0; i < nb; i++) {
+        if (!mask[b0 + i]) continue;
+        for (size_t e = 0; e < nw; e++) dst[(size_t)i * nw + e] = (double)src[(size_t)i * nw + e];
+        if (tau_out)
+          for (int j = 0; j < 10; j++) tau_out[(size_t)(b0 + i) * 10 + j] = (double)ht[(size_t)i * 10 + j];
+        if (status) status[b0 + i] = hst[i];
+        if (HMPC_STATUS_CODE(hst[i]) != 0) all_ok = false;
+      }
+      continue;
+    }
+    if (tau_out)
+      for (int i = 0; i < nb * 10; i++) tau_out[(size_t)b0 * 10 + i] = (double)ht[i];
     const size_t tot = (size_t)nb * nw;
     if (c->pool && nb >= 128) {
       c->pool->parallel([&](int part, int nparts) {

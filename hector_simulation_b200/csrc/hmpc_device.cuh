@@ -2363,4 +2363,42 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Masked solve (hmpc_solve_device_masked): robot i is solved iff mask[i] != 0.  This kernel turns the mask into class 0's
+// instance list, in ascending robot order, and its length word.  One CTA scans the mask in tiles of NT bytes: a ballot
+// and popc inside each warp, the warp totals through shared memory across warps.  A single CTA writes the list in order
+// without a second pass, and it runs as it is in the host emulation.  At 4096 robots it is 8 tiles.
+// ------------------------------------------------------------------------------------------------
+constexpr int SELECT_THREADS = 512;
+
+template <int NT>
+__global__ void __launch_bounds__(NT) hmpc_select_kernel(const unsigned char* mask, int batch, int* list, int* count)
+{
+  constexpr int NW = NT / 32;
+  __shared__ int wtot[NW];
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  pdl_trigger();  // class 0 may become resident; it waits for this kernel before it reads the list
+  // The previous call's class-0 launch clears the length words this call uses, and the kernel before this one may have
+  // written the mask: nothing is read or stored before both have completed.
+  pdl_wait();
+  int base = 0;
+  for (int t0 = 0; t0 < batch; t0 += NT) {
+    const int i = t0 + tid;
+    const bool on = i < batch && mask[i] != 0;
+    const unsigned bal = __ballot_sync(0xffffffffu, on);
+    if (lane == 0) wtot[wid] = __popc(bal);
+    __syncthreads();
+    int off = base, tot = 0;
+    for (int w = 0; w < NW; w++) {
+      const int n = wtot[w];
+      off += w < wid ? n : 0;
+      tot += n;
+    }
+    if (on) list[off + __popc(bal & ((1u << lane) - 1u))] = i;
+    base += tot;
+    __syncthreads();  // the next tile rewrites wtot
+  }
+  if (tid == 0) *count = base;
+}
+
 }  // namespace hmpc

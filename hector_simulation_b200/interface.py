@@ -31,6 +31,7 @@ EXPORTS = [
     "hmpc_reference_last_status", "hmpc_reference_last_rc",
     "hmpc_solve_device_warm", "hmpc_solve_batch_warm", "hmpc_reference_set_warm_start",
     "hmpc_set_refinement", "hmpc_reference_set_refinement",
+    "hmpc_solve_device_masked", "hmpc_solve_batch_masked",
 ]
 REFINEMENT_CLASS = 3  # hmpc_class_config index of the refinement class (HMPC_REFINEMENT_CLASS)
 
@@ -119,6 +120,10 @@ def lib() -> ctypes.CDLL:
         L.hmpc_set_refinement.restype = ctypes.c_int
         L.hmpc_reference_set_refinement.argtypes = [ctypes.c_int]
         L.hmpc_reference_set_refinement.restype = None
+        L.hmpc_solve_device_masked.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 6
+        L.hmpc_solve_device_masked.restype = ctypes.c_int
+        L.hmpc_solve_batch_masked.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 5
+        L.hmpc_solve_batch_masked.restype = ctypes.c_int
         _lib = L
     return _lib
 
@@ -325,6 +330,34 @@ class BatchedMPC:
                allow_not_converged=not strict)
         return (wrench, tau, status) if torques else (wrench, status)
 
+    def solve_batch_masked(self, records: np.ndarray, mask, shift=None, torques: bool = False, strict: bool = True, out=None):
+        """solve_batch_warm of the robots with mask[i] != 0 only (hmpc_solve_batch_masked): `mask` bool or uint8 [B], `shift`
+        int32 [B] read for listed robots only (None: 1 each).  Only listed rows of the results are written.  With out=None the
+        arrays are new and unlisted rows hold zeros (a status of 0 there means "not solved", not "optimal"); with
+        `out=(wrench, status)` they keep what the caller's arrays held.  strict: raise when a listed robot did not converge.
+        -> (wrench, status), or (wrench, tau, status) with torques=True."""
+        if records.dtype != UPDATE_DTYPE or not records.flags.c_contiguous:
+            records = np.ascontiguousarray(records, dtype=UPDATE_DTYPE)
+        B = records.shape[0]
+        mask = np.ascontiguousarray(np.asarray(mask) != 0).view(np.uint8)
+        assert mask.shape == (B,)
+        if out is not None:
+            wrench, status = out
+            assert wrench.dtype == np.float64 and wrench.shape == (B, 12 * self.horizon) and wrench.flags.c_contiguous
+            assert status.dtype == np.int32 and status.shape == (B,)
+        else:
+            wrench = np.zeros((B, 12 * self.horizon), dtype=np.float64)
+            status = np.zeros(B, dtype=np.int32)
+        tau = np.zeros((B, 10), dtype=np.float64) if torques else None
+        if shift is not None:
+            shift = np.ascontiguousarray(shift, dtype=np.int32)
+            assert shift.shape == (B,)
+        _check(lib().hmpc_solve_batch_masked(self._h, records.ctypes.data, B, mask.ctypes.data, wrench.ctypes.data,
+                                             tau.ctypes.data if torques else None, status.ctypes.data,
+                                             shift.ctypes.data if shift is not None else None),
+               allow_not_converged=not strict)
+        return (wrench, tau, status) if torques else (wrench, status)
+
     def solve_batch_torques(self, records: np.ndarray, strict: bool = True):
         """Host path with the leg-controller epilogue: -> (wrench [B,12N], tau [B,10], status [B])."""
         records = np.ascontiguousarray(records, dtype=UPDATE_DTYPE)
@@ -437,6 +470,18 @@ class BatchedMPC:
         _check(lib().hmpc_solve_device_warm(self._h, d_records.data_ptr(), B, d_wrench.data_ptr(), d_status.data_ptr(),
                                             d_tau.data_ptr() if d_tau is not None else None,
                                             d_shift.data_ptr() if d_shift is not None else None, ctypes.c_void_p(st)))
+
+    def solve_device_masked(self, d_records, B: int, d_mask, d_wrench, d_status, d_tau=None, d_shift=None, stream=None) -> None:
+        """solve_device_warm of the robots with d_mask[i] != 0 only (hmpc_solve_device_masked).  `d_mask` torch bool or uint8
+        [B] on the GPU, read on the device: no host synchronisation.  Unlisted rows of d_wrench, d_status, d_tau and their
+        working sets keep their bytes.  Capturable in a CUDA graph: a replay solves the robots the captured mask lists
+        when it runs."""
+        import torch
+
+        st = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        _check(lib().hmpc_solve_device_masked(self._h, d_records.data_ptr(), B, d_mask.data_ptr(), d_wrench.data_ptr(),
+                                              d_status.data_ptr(), d_tau.data_ptr() if d_tau is not None else None,
+                                              d_shift.data_ptr() if d_shift is not None else None, ctypes.c_void_p(st)))
 
     def assemble_device(self, d_records, B: int, stream=None) -> dict:
         """Parity hook: un-reduced fp32 QP data of B packed records (torch tensors on the GPU)."""

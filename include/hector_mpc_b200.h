@@ -257,6 +257,27 @@ HMPC_EXTERNC int hmpc_solve_device_warm(hmpc_ctx* ctx, const void* d_records, in
                                         float* d_tau, const int* d_shift, void* stream);
 HMPC_EXTERNC int hmpc_solve_batch_warm(hmpc_ctx* ctx, const struct update_data_t* in, int B, double* wrench_out,
                                        double* tau_out, int* status, const int* shift);
+/* Solving part of the batch.  A reference-style controller runs its MPC only every iterationsBetweenMPC control ticks
+ * of each robot's own counter (ConvexMPCLocomotion.cpp:277), and robots that stand, lie or wait for a reset need none,
+ * so in a batch of robots reset at different times only a changing subset is due in any tick.  The masked calls solve
+ * robot i iff mask[i] != 0 (a torch.bool tensor can be passed as it is), with the arrays sized for the whole batch:
+ * records, outputs, mask[B] and shift[B], B <= the context's capacity.
+ *   - A listed robot's wrench row, status word, torque row and working-set slot are written exactly as the _warm call
+ *     writes them.  An unlisted robot's keep their bytes, on the host arrays too in every host-buffer mode.
+ *   - Warm start as in the _warm calls: slot i is robot i, whatever other robots are listed; shift[i] (read for listed
+ *     robots only) is the MPC steps robot i's horizon moved since its last solve on this context.  NULL = 1 for every
+ *     listed robot, 0 = the same horizon, < 0 = a cold solve that records the set.  HMPC_WARM_START=0 and
+ *     hmpc_set_refinement act as in the other calls.
+ *   - An empty mask is valid: nothing is written.  The host call returns HMPC_ERR_NOT_CONVERGED for listed robots only.
+ *   - Argument checks as in the _warm calls, plus a NULL mask is HMPC_ERR_ARG; B = 0 is a no-op.
+ *   hmpc_solve_device_masked: as hmpc_solve_device_warm; d_mask device bytes [B].  The mask is read on the device, by one
+ *                             more launch ahead of the chain, so the call needs no host synchronisation and one captured
+ *                             graph serves every mask written into the captured buffer.
+ *   hmpc_solve_batch_masked : as hmpc_solve_batch_warm (all three host-buffer modes); mask host bytes [B]. */
+HMPC_EXTERNC int hmpc_solve_device_masked(hmpc_ctx* ctx, const void* d_records, int B, const unsigned char* d_mask,
+                                          float* d_wrench, int* d_status, float* d_tau, const int* d_shift, void* stream);
+HMPC_EXTERNC int hmpc_solve_batch_masked(hmpc_ctx* ctx, const struct update_data_t* in, int B, const unsigned char* mask,
+                                         double* wrench_out, double* tau_out, int* status, const int* shift);
 /* The reference boundary warm-started: after hmpc_reference_set_warm_start(1), every update_problem_data proposes the
  * previous call's working set moved one step (a hmpc_solve_batch_warm with shift NULL on the one-robot context).
  * setup_problem with another dt, f_max or horizon forgets it.  Default 0: every tick a cold start, like the reference. */
@@ -317,8 +338,8 @@ HMPC_EXTERNC int hmpc_swing_device(hmpc_ctx* ctx, const struct hmpc_state_t* d_s
 
 /* CUDA graphs.  The device-resident calls can be recorded into a CUDA graph by stream capture (cudaStreamBeginCapture,
  * torch.cuda.graph, ...) on the stream they are given: hmpc_solve_device, hmpc_solve_device_ex, hmpc_solve_device_warm,
- * hmpc_prepare_device, hmpc_rollout_device, hmpc_swing_device and hmpc_reset_warm_start.  Each launch of the graph gives
- * the results an eager call on the same inputs gives, bit for bit.
+ * hmpc_solve_device_masked, hmpc_prepare_device, hmpc_rollout_device, hmpc_swing_device and hmpc_reset_warm_start.  Each
+ * launch of the graph gives the results an eager call on the same inputs gives, bit for bit.
  *   - A replay is a real call.  A captured warm solve proposes and records working sets, a captured rollout advances
  *     d_states and d_loop, a captured hmpc_reset_warm_start clears the working sets, every time the graph is launched.
  *   - A context's calls, eager ones and graph launches alike, must be ordered on one stream (or by events).  All chains
@@ -328,7 +349,7 @@ HMPC_EXTERNC int hmpc_swing_device(hmpc_ctx* ctx, const struct hmpc_state_t* d_s
  *   - A graph must not be launched after hmpc_destroy of its context.
  *   - A call that returns an error while its stream is capturing may have recorded part of its work: end the capture
  *     and discard the graph.  Argument errors are found before anything is enqueued.
- * The host-buffer calls (hmpc_solve_batch, _ex, _warm, _states, hmpc_solve_batch_sharded) and the reference boundary
+ * The host-buffer calls (hmpc_solve_batch, _ex, _warm, _masked, _states, hmpc_solve_batch_sharded) and the reference boundary
  * (update_problem_data) wait for their own streams and cannot be captured. */
 
 /* Robots beyond the conditioning limit (INTEGRATION.md).  The fp64 sweep inversion of the solve is accurate up to a scaled
