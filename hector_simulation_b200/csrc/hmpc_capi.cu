@@ -23,6 +23,7 @@
 
 #include "../../include/hector_mpc_b200.h"
 #include "hmpc_device.cuh"
+#include "hmpc_chain.h"
 
 static_assert(sizeof(update_data_t) == 3016, "update_data_t must match convexMPC_interface.h:19-37");
 static_assert(sizeof(problem_setup) == 16, "problem_setup must match convexMPC_interface.h:11-17");
@@ -117,46 +118,36 @@ class HostPool {
 
 constexpr int NCHUNK = 4;  // the host-buffer path pipelines pack / H2D / solve / D2H over this many chunks
 
-// ints of one slot of hmpc_ctx::d_cls: [2 parities x 8 words | class-1 list | class-2 list | refinement list | class-0 list]
-size_t cls_slot_ints(int max_batch) { return 16 + 4 * (size_t)max_batch; }
-
-struct ClassCfg {
-  int nb_hi, nb_cap, qmax, threads, smem, grid_cap, variant, tcap;
-  hmpc::Layout L;
-};
+using hmpc::ClassCfg;
 
 }  // namespace
 
 struct hmpc_ctx {
   int device = 0, max_batch = 0, horizon = 0, rec_stride = 0, sm_count = 0;
-  problem_setup setup{};
+  hmpc::SolverSettings cfg;
   ClassCfg cls[3];
   int ncls = 0;
   // refinement class (hmpc_set_refinement): instances beyond the conditioning limit are solved again with iterative
   // refinement against the stored Hessian instead of ending with code 4
   ClassCfg ref{};
-  int refine = 0;
-  double kappa_refine = 1.5e4;   // hand-over threshold of classes 0-2 while refinement is on (HMPC_KAPPA_REFINE; DESIGN.md §2)
-  double kappa_max_refined = 1e9;  // conditioning limit of the refinement class (HMPC_KAPPA_MAX_REFINED)
   int* d_ref = nullptr;            // host-buffer path: [NCHUNK][1 + max_batch] refinement list length + list
   unsigned char* d_rec = nullptr;
   unsigned char* d_out = nullptr;  // host-buffer path: per chunk [wrench floats | status ints], contiguous
   int* d_status = nullptr;         // scratch status (assembly hook)
-  int* d_counts = nullptr;         // [NCHUNK][2] class list lengths
-  int* d_lists = nullptr;          // [NCHUNK][2][max_batch] class lists (host-built, host-buffer path)
-  int* d_cls = nullptr;            // [NCHUNK][cls_slot_ints] class-list lengths and lists (device-resident path;
-                                   // slot 0: eager chains, slot 1: chains recorded into a CUDA graph)
+  int* d_counts = nullptr;         // [NCHUNK][4] class list lengths (assembly hook)
+  int* d_lists = nullptr;          // [NCHUNK][host_lists_ints] class lists (host-built, host-buffer path)
+  int* d_cls = nullptr;            // [NCHUNK][ClassSlot::cls_slot_ints] class-list lengths and lists (device-resident
+                                   // path; slot 0: eager chains, slot 1: chains recorded into a CUDA graph)
   unsigned char* h_mask = nullptr; // pinned [max_batch]: the mask of hmpc_solve_batch_masked, read mapped by the in-place mode
   unsigned tick[NCHUNK] = {0, 0, 0, 0};  // eager calls per slot: parity of the list lengths in use
   unsigned char* h_rec = nullptr;  // pinned
   unsigned char* h_out = nullptr;  // pinned mirror of d_out
   unsigned char* d_states = nullptr;  // hmpc_state_t staging of hmpc_solve_batch_states (row f-1)
   unsigned char* h_states = nullptr;  // pinned
-  int* h_cls = nullptr;            // pinned [NCHUNK][4 + 3*max_batch]: host-built class counts + lists (host-buffer path)
+  int* h_cls = nullptr;            // pinned [NCHUNK][host_lists_ints]: host-built class counts + lists (host-buffer path)
   cudaStream_t stream = nullptr;   // chunk 0 / single-robot stream
   cudaStream_t xstream[3] = {nullptr, nullptr, nullptr};  // further chunks of the pipelined host path
   HostPool* pool = nullptr;        // helper threads for packing / widening (large batches only)
-  int max_iter = 500;  // same cap as the reference's nWSR (SolverMPC.cpp:584)
   // multi-GPU (one process per GPU, batch sharded): NCCL communicator + double-buffered float results for the gather
   void* nccl = nullptr;            // ncclComm_t
   int shard_rank = 0, shard_world = 1;
@@ -170,10 +161,6 @@ struct hmpc_ctx {
   int warm_start = 1;              // the warm calls propose them to the next tick (HMPC_WARM_START=0: cold start every tick)
   int* d_shift = nullptr;          // [max_batch] per-robot shifts of hmpc_solve_batch_warm (staged copy)
   int* h_shift = nullptr;          // pinned [max_batch] the same, also read mapped by the zero-copy and in-place modes
-  int lockstep = 1;                // waves of a multi-wave launch start together (HMPC_LOCKSTEP=0: free-running, for A/B runs)
-  double kappa_max = 1.5e5;  // conditioning limit of the fp64 sweep inversion (HMPC_KAPPA_MAX; see the kernel's stage 5)
-  int block_min = 2;     // later rounds need at least this many entering rows (HMPC_BLOCK_MIN, A/B knob)
-  int block_rounds = 4;  // block start of the active-set stage (HMPC_BLOCK_ROUNDS=0: plain dual iteration, for A/B runs)
   // caller-owned host buffers registered with hmpc_pin_host_buffer: hmpc_solve_batch lets the kernels read the
   // reference records from them and write results to them in place (no packing, no staging copies, no widening)
   struct Pin { char* base; size_t bytes; };   // what the caller asked for
@@ -191,46 +178,20 @@ struct hmpc_ctx {
 
 namespace {
 
-// kernel variants <threads, min CTAs/SM, fixed horizon (0 = runtime), size class>
-//   0/1: horizon 10 fixed at compile time (class 0: 4 warps, 6 CTAs/SM — shared memory would allow 7, but at 7 the
-//        register budget of 72 spills more and the 1024-robot batch was slower on the H100; class 1: 8 warps)
-//   10 + 5*cls + b: runtime horizon, b-th entry of {64, 128, 192, 256, 384} threads
-//   20 + b: the refinement class, b-th entry of the same (one CTA per SM: it is rare and its shared memory is large)
-#define HMPC_FOR_VARIANT(V, X)                   \
-  switch (V) {                                   \
-    case 0: X(128, 6, 10, 0); break;             \
-    case 1: X(256, 2, 10, 1); break;             \
-    case 20: X(64, 1, 0, 3); break;              \
-    case 21: X(128, 1, 0, 3); break;             \
-    case 22: X(192, 1, 0, 3); break;             \
-    case 23: X(256, 1, 0, 3); break;             \
-    case 24: X(384, 1, 0, 3); break;             \
-    case 10: X(64, 8, 0, 0); break;              \
-    case 11: X(128, 6, 0, 0); break;             \
-    case 12: X(192, 3, 0, 0); break;             \
-    case 13: X(256, 2, 0, 0); break;             \
-    case 14: X(384, 1, 0, 0); break;             \
-    case 15: X(64, 8, 0, 1); break;              \
-    case 16: X(128, 6, 0, 1); break;             \
-    case 17: X(192, 3, 0, 1); break;             \
-    case 18: X(256, 2, 0, 1); break;             \
-    default: X(384, 1, 0, 1); break;             \
-  }
-const int kBucketThreads[5] = {64, 128, 192, 256, 384};
-
-cudaError_t prep_class(ClassCfg& c, int* occ)
+cudaError_t prep_class(const ClassCfg& c, int* occ)
 {
-  cudaError_t e = cudaSuccess;
+  cudaError_t e = cudaErrorInvalidDeviceFunction;
   // The attribute is per kernel instantiation and process-wide, and several contexts (other horizons, the
   // reference-style global context) share the runtime-horizon instantiations: always raise it to the device's opt-in
   // maximum instead of this context's carve-up, so no context can lower it under another's launches.
-#define HMPC_PREP(NT, MB, NF, CL)                                                                       \
-  {                                                                                                    \
+#define HMPC_PREP(ID, NT, MB, NF, CL)                                                                   \
+  case ID: {                                                                                           \
     auto k = hmpc::hmpc_solve_kernel<NT, MB, NF, CL>;                                                  \
     e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);              \
     if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, k, NT, c.smem);       \
+    break;                                                                                             \
   }
-  HMPC_FOR_VARIANT(c.variant, HMPC_PREP)
+  switch (c.variant) { HMPC_VARIANTS(HMPC_PREP) }
 #undef HMPC_PREP
   return e;
 }
@@ -260,67 +221,13 @@ cudaError_t launch_chain(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t
   return cudaLaunchKernelEx(&cfg, kernel, args...);
 }
 
-cudaError_t launch_class(const ClassCfg& c, const hmpc::KernelArgs& ka, int grid, cudaStream_t st, bool pdl = false)
-{
-  cudaError_t e = cudaSuccess;
-#define HMPC_LAUNCH(NT, MB, NF, CL) \
-  e = launch_chain(hmpc::hmpc_solve_kernel<NT, MB, NF, CL>, dim3(grid), dim3(NT), (size_t)c.smem, st, pdl, ka);
-  HMPC_FOR_VARIANT(c.variant, HMPC_LAUNCH)
-#undef HMPC_LAUNCH
-  return e != cudaSuccess ? e : cudaGetLastError();
-}
-
+// the shapes of the context's classes (hmpc::plan_classes) and what the device makes of them: resident CTAs per class
 int build_classes(hmpc_ctx* c)
 {
-  const int N = c->horizon;
-  // class 0: at most N blocks of 6 variables (e.g. any single-support schedule); class 1: up to 2N.
-  // Working-set overflow in class 0 escalates to class 1.
-  // class 2 = class 1's size with as many working-set slots as one SM's shared memory holds (1 CTA/SM): reached only
-  // by escalation from class 1 (massively degenerate optima, e.g. all contact forces at zero).
-  c->ncls = 3;
-  for (int i = 0; i < 3; i++) {
-    ClassCfg& k = c->cls[i];
-    if (i == 2) {
-      // class 2: class 1's size, every row may be active; no H^-1 a_j cache (its primal steps go through a full product)
-      k = c->cls[1];
-      const int n = 6 * k.nb_cap;
-      if (c->cls[1].qmax >= n) { c->ncls = 2; break; }  // class 1 already holds every row
-      k.qmax = n;
-      k.tcap = 0;
-      if (N == 10) {  // the runtime-layout instantiation of the same shape (the fixed one folds class 1's layout)
-        k.variant = 18;
-        k.threads = 256;
-      }
-      k.L = hmpc::make_layout(N, k.nb_cap, k.qmax, c->rec_stride, k.threads / 32, 0);
-      while (k.L.total > 226 * 1024 && k.qmax > c->cls[1].qmax) {
-        k.qmax -= 4;
-        k.L = hmpc::make_layout(N, k.nb_cap, k.qmax, c->rec_stride, k.threads / 32, 0);
-      }
-      if (k.qmax <= c->cls[1].qmax) { c->ncls = 2; break; }
-      k.smem = k.L.total;
-      int occ = 0;
-      if (cuda_fail(prep_class(k, &occ), "kernel attribute/occupancy (class 2)")) return HMPC_ERR_CUDA;
-      if (occ < 1) { g_err = "class-2 kernel does not fit on this device"; return HMPC_ERR_CUDA; }
-      k.grid_cap = occ * c->sm_count;
-      break;
-    }
-    k.nb_cap = hmpc::class_nb_cap(N, i);
-    k.nb_hi = k.nb_cap;
-    const int warps = hmpc::class_warps(N, i);
-    int bucket = 0;
-    while (bucket < 4 && kBucketThreads[bucket] < 32 * warps) bucket++;
-    if (kBucketThreads[bucket] < 32 * warps) { g_err = "horizon too long for the built kernel variants"; return HMPC_ERR_ARG; }
-    if (N == 10) {
-      k.variant = i;
-      k.threads = (i == 0) ? 128 : 256;
-    } else {
-      k.variant = 10 + 5 * i + bucket;
-      k.threads = kBucketThreads[bucket];
-    }
-    k.qmax = hmpc::class_qmax(N, i);
-    k.tcap = hmpc::class_tcap(N, i);
-    k.L = hmpc::make_layout(N, k.nb_cap, k.qmax, c->rec_stride, k.threads / 32, k.tcap);
-    k.smem = k.L.total;
+  c->ncls = hmpc::plan_classes(c->horizon, c->cls, c->ref);
+  if (c->ncls == 0) { g_err = "horizon too long for the built kernel variants"; return HMPC_ERR_ARG; }
+  for (int i = 0; i <= c->ncls; i++) {
+    ClassCfg& k = i < c->ncls ? c->cls[i] : c->ref;
     int occ = 0;
     if (cuda_fail(prep_class(k, &occ), "kernel attribute/occupancy (is this an sm_90a device?)")) return HMPC_ERR_CUDA;
     if (occ < 1) { g_err = "kernel does not fit on this device"; return HMPC_ERR_CUDA; }
@@ -329,92 +236,24 @@ int build_classes(hmpc_ctx* c)
   return HMPC_OK;
 }
 
-// The refinement class (hmpc_set_refinement): class 2's shape — no column cache, as many working-set slots as shared memory
-// holds — plus the float32 H tiles and g that its refinement rounds read (refine_layout).  It holds double support (2N
-// blocks) while that leaves at least class 1's working-set capacity, i.e. up to horizon 14; beyond that single support
-// (N blocks), and an instance with more stance blocks keeps its code 4.
-int build_refine_class(hmpc_ctx* c)
+long long* g_dbg_clk = nullptr;  // profiling hook (hmpc_debug_set_clock_buffer)
+
+// one launch of class `cls` (0-2, or hmpc::REFINE_CLASS) over `count` instances, as many CTAs as are resident at most
+int launch_class(const hmpc_ctx* c, int cls, const hmpc::SolveIO& io, const hmpc::ChainLists& lists, int count, cudaStream_t st,
+                 bool pdl = false)
 {
-  const int N = c->horizon;
-  ClassCfg& k = c->ref;
-  for (int nb = 2 * N;; nb = N) {
-    const int n = 6 * nb, nt8 = (n + 7) / 8;
-    const int w_sweep = (nt8 + 1) / 2, w_rows = (nb + 2) / 3, warps = w_sweep > w_rows ? w_sweep : w_rows;
-    int bucket = 0;
-    while (bucket < 4 && kBucketThreads[bucket] < 32 * warps) bucket++;
-    k.nb_cap = k.nb_hi = nb;
-    k.variant = 20 + bucket;
-    k.threads = kBucketThreads[bucket];
-    k.tcap = 0;
-    k.qmax = n;
-    k.L = hmpc::refine_layout(N, nb, k.qmax, c->rec_stride, k.threads / 32);
-    while (k.L.total > 226 * 1024 && k.qmax > 4) {
-      k.qmax -= 4;
-      k.L = hmpc::refine_layout(N, nb, k.qmax, c->rec_stride, k.threads / 32);
-    }
-    if (nb == N || (k.L.total <= 226 * 1024 && k.qmax >= hmpc::class_qmax(N, 1))) break;
-  }
-  k.smem = k.L.total;
-  int occ = 0;
-  if (cuda_fail(prep_class(k, &occ), "kernel attribute/occupancy (refinement class)")) return HMPC_ERR_CUDA;
-  if (occ < 1) { g_err = "refinement-class kernel does not fit on this device"; return HMPC_ERR_CUDA; }
-  k.grid_cap = occ * c->sm_count;
+  const ClassCfg& k = cls == hmpc::REFINE_CLASS ? c->ref : c->cls[cls];
+  hmpc::KernelArgs ka = hmpc::launch_args(c->cfg, c->horizon, c->ncls, cls, k, io, lists);
+  ka.dbg_clk = ka.dbg_H ? nullptr : g_dbg_clk;  // (the assembly dump is not stamped)
+  const int grid = count < k.grid_cap ? count : k.grid_cap;
+  cudaError_t e = cudaErrorInvalidDeviceFunction;
+#define HMPC_LAUNCH(ID, NT, MB, NF, CL) \
+  case ID: e = launch_chain(hmpc::hmpc_solve_kernel<NT, MB, NF, CL>, dim3(grid), dim3(NT), (size_t)k.smem, st, pdl, ka); break;
+  switch (k.variant) { HMPC_VARIANTS(HMPC_LAUNCH) }
+#undef HMPC_LAUNCH
+  CK(e);
+  CK(cudaGetLastError());
   return HMPC_OK;
-}
-
-// the hand-over threshold of classes 0-2: the refinement threshold while refinement is on, else the conditioning limit
-double kappa_handover(const hmpc_ctx* c) { return c->refine ? c->kappa_refine : c->kappa_max; }
-
-// arguments of a refinement-class launch over `list` (length at *count, device memory)
-hmpc::KernelArgs refine_args(const hmpc_ctx* c, const void* d_records, const update_data_t* raw, int B, float* d_wrench32,
-                             double* d_wrench64, int* d_status, float* d_tau, int* d_ws, const int* list, int* count)
-{
-  const ClassCfg& k = c->ref;
-  hmpc::KernelArgs ka{};
-  ka.records = static_cast<const unsigned char*>(d_records);
-  ka.raw_records = reinterpret_cast<const unsigned char*>(raw);
-  ka.rec_stride = c->rec_stride;
-  ka.batch = B;
-  ka.horizon = c->horizon;
-  ka.dt = c->setup.dt;
-  ka.f_max = c->setup.f_max;
-  ka.max_iter = c->max_iter;
-  ka.tol_kkt = 1e-9;
-  ka.tol_dep = 1e-11;
-  ka.kappa_max = c->kappa_max_refined;
-  ka.wrench = d_wrench32;
-  ka.wrench64 = d_wrench64;
-  ka.status = d_status;
-  ka.tau = d_tau;
-  ka.ws_state = d_ws;  // warm_start 0: no proposal; the class records an empty set
-  ka.list = list;
-  ka.counts = count;   // counts[cls] with cls 0
-  ka.split_nb = -1;
-  ka.nb_cap = k.nb_cap;
-  ka.qmax = k.qmax;
-  ka.tcap = 0;
-  ka.L = k.L;
-  return ka;
-}
-
-hmpc::KernelArgs base_args(const hmpc_ctx* c, const void* d_records, int B, float* d_wrench, int* d_status)
-{
-  hmpc::KernelArgs ka{};
-  ka.records = static_cast<const unsigned char*>(d_records);
-  ka.rec_stride = c->rec_stride;
-  ka.batch = B;
-  ka.horizon = c->horizon;
-  ka.dt = c->setup.dt;
-  ka.f_max = c->setup.f_max;
-  ka.max_iter = c->max_iter;
-  ka.tol_kkt = 1e-9;
-  ka.tol_dep = 1e-11;
-  ka.block_rounds = c->block_rounds;
-  ka.block_min = c->block_min;
-  ka.kappa_max = kappa_handover(c);
-  ka.wrench = d_wrench;
-  ka.status = d_status;
-  return ka;
 }
 
 }  // namespace
@@ -639,10 +478,6 @@ HMPC_EXTERNC hmpc_ctx* hmpc_create(int max_batch, int horizon, int device)
   c->max_batch = max_batch;
   c->horizon = horizon;
   c->rec_stride = (int)hmpc_record_bytes(horizon);
-  c->setup.dt = 0.04f;
-  c->setup.mu = 0.25f;
-  c->setup.f_max = 500.f;
-  c->setup.horizon = horizon;
   cudaDeviceProp prop{};
   bool bad = cuda_fail(cudaSetDevice(device), "cudaSetDevice") ||
              cuda_fail(cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties");
@@ -661,32 +496,32 @@ HMPC_EXTERNC hmpc_ctx* hmpc_create(int max_batch, int horizon, int device)
           cuda_fail(cudaMalloc(&c->d_rec, (size_t)max_batch * c->rec_stride), "cudaMalloc records") ||
           cuda_fail(cudaMalloc(&c->d_out, (size_t)max_batch * (nw * 4 + 4 + 40)), "cudaMalloc results") ||
           cuda_fail(cudaMalloc(&c->d_counts, NCHUNK * 4 * sizeof(int)), "cudaMalloc counts") ||
-          cuda_fail(cudaMalloc(&c->d_lists, (size_t)NCHUNK * (4 + 3 * (size_t)max_batch) * sizeof(int)), "cudaMalloc lists") ||
+          cuda_fail(cudaMalloc(&c->d_lists, (size_t)NCHUNK * hmpc::host_lists_ints(max_batch) * sizeof(int)), "cudaMalloc lists") ||
           cuda_fail(cudaMalloc(&c->d_ws, (size_t)max_batch * hmpc::WS_STATE_INTS * sizeof(int)), "cudaMalloc working sets") ||
           cuda_fail(cudaMemset(c->d_ws, 0, (size_t)max_batch * hmpc::WS_STATE_INTS * sizeof(int)), "cudaMemset working sets") ||
           cuda_fail(cudaMalloc(&c->d_shift, (size_t)max_batch * sizeof(int)), "cudaMalloc shifts") ||
           cuda_fail(cudaMallocHost(&c->h_shift, (size_t)max_batch * sizeof(int)), "cudaMallocHost shifts") ||
           cuda_fail(cudaMallocHost(&c->h_mask, (size_t)max_batch), "cudaMallocHost mask") ||
-          cuda_fail(cudaMalloc(&c->d_cls, (size_t)NCHUNK * cls_slot_ints(max_batch) * sizeof(int)), "cudaMalloc class lists") ||
-          cuda_fail(cudaMemset(c->d_cls, 0, (size_t)NCHUNK * cls_slot_ints(max_batch) * sizeof(int)), "cudaMemset class lists") ||
+          cuda_fail(cudaMalloc(&c->d_cls, (size_t)NCHUNK * hmpc::ClassSlot::cls_slot_ints(max_batch) * sizeof(int)), "cudaMalloc class lists") ||
+          cuda_fail(cudaMemset(c->d_cls, 0, (size_t)NCHUNK * hmpc::ClassSlot::cls_slot_ints(max_batch) * sizeof(int)), "cudaMemset class lists") ||
           cuda_fail(cudaMalloc(&c->d_ref, (size_t)NCHUNK * (1 + (size_t)max_batch) * sizeof(int)), "cudaMalloc refinement lists") ||
           cuda_fail(cudaMalloc(&c->d_status, (size_t)max_batch * 4), "cudaMalloc status") ||
           cuda_fail(cudaMalloc(&c->d_states, (size_t)max_batch * sizeof(hmpc_state_t)), "cudaMalloc states") ||
           cuda_fail(cudaMallocHost(&c->h_states, (size_t)max_batch * sizeof(hmpc_state_t)), "cudaMallocHost states") ||
           cuda_fail(cudaMallocHost(&c->h_rec, (size_t)max_batch * c->rec_stride), "cudaMallocHost records") ||
           cuda_fail(cudaMallocHost(&c->h_out, (size_t)max_batch * (nw * 4 + 4 + 40)), "cudaMallocHost results") ||
-          cuda_fail(cudaMallocHost(&c->h_cls, (size_t)NCHUNK * (4 + 3 * (size_t)max_batch) * sizeof(int)), "cudaMallocHost lists") ||
-          build_classes(c) != HMPC_OK || build_refine_class(c) != HMPC_OK;
+          cuda_fail(cudaMallocHost(&c->h_cls, (size_t)NCHUNK * hmpc::host_lists_ints(max_batch) * sizeof(int)), "cudaMallocHost lists") ||
+          build_classes(c) != HMPC_OK;
   }
   if (!bad) {
     const char* br = getenv("HMPC_BLOCK_ROUNDS");
-    if (br) c->block_rounds = atoi(br);
-    if (const char* bm = getenv("HMPC_BLOCK_MIN")) c->block_min = atoi(bm);
-    if (const char* km = getenv("HMPC_KAPPA_MAX")) c->kappa_max = atof(km);
-    if (const char* kr = getenv("HMPC_KAPPA_REFINE")) c->kappa_refine = atof(kr);
-    if (const char* kx = getenv("HMPC_KAPPA_MAX_REFINED")) c->kappa_max_refined = atof(kx);
+    if (br) c->cfg.block_rounds = atoi(br);
+    if (const char* bm = getenv("HMPC_BLOCK_MIN")) c->cfg.block_min = atoi(bm);
+    if (const char* km = getenv("HMPC_KAPPA_MAX")) c->cfg.kappa_max = atof(km);
+    if (const char* kr = getenv("HMPC_KAPPA_REFINE")) c->cfg.kappa_refine = atof(kr);
+    if (const char* kx = getenv("HMPC_KAPPA_MAX_REFINED")) c->cfg.kappa_max_refined = atof(kx);
     const char* ls = getenv("HMPC_LOCKSTEP");
-    if (ls) c->lockstep = atoi(ls);
+    if (ls) c->cfg.lockstep = atoi(ls);
     const char* wm = getenv("HMPC_WARM_START");
     if (wm) c->warm_start = atoi(wm);
   }
@@ -710,170 +545,88 @@ HMPC_EXTERNC int hmpc_set_problem(hmpc_ctx* c, const problem_setup* s)
 {
   if (!c || !s) { g_err = "hmpc_set_problem: null argument"; return HMPC_ERR_ARG; }
   if (s->horizon != c->horizon) { g_err = "hmpc_set_problem: horizon differs from the context's"; return HMPC_ERR_ARG; }
-  c->setup = *s;
+  c->cfg.dt = s->dt;
+  c->cfg.f_max = s->f_max;
   return HMPC_OK;
 }
 
 namespace {
-long long* g_dbg_clk = nullptr;  // profiling hook (hmpc_debug_set_clock_buffer)
 // The slot of d_cls whose list lengths a chain recorded into a CUDA graph uses.  Eager chains use slot 0.
 constexpr int CAPTURE_SLOT = 1;
 static_assert(CAPTURE_SLOT < NCHUNK, "d_cls holds NCHUNK slots");
-// one launch per class, all enqueued on `st`; with `mask` (device-readable [B]) the selection kernel first
-int enqueue_solve(hmpc_ctx* c, const void* d_records, int B, float* d_wrench32, double* d_wrench64, int* d_status,
-                  cudaStream_t st, int slot = 0, float* d_tau = nullptr, int* d_ws = nullptr, int ws_shift = 0, bool ws_read = false,
-                  const update_data_t* raw = nullptr, const int* ws_shifts = nullptr, const unsigned char* mask = nullptr)
+// The device-resident chain: one launch per class, all enqueued on `st`; with io.mask (device-readable [B]) the selection
+// kernel first.  No classification kernel: the class-0 launch runs over every instance (or, in a masked call, over the list
+// the selection kernel built from the mask) and hands the ones with more stance blocks than it holds to class 1's list.
+// An eager chain uses the parity of its call count: the previous call's class-0 launch zeroed those lengths.  A graph
+// replays the lengths it was recorded with and nothing zeroes them between replays, so a chain recorded into a graph
+// uses the capture slot, starts with a memset node that zeroes both parities (the wave-barrier counter and the
+// refinement list length included), and leaves the eager call count alone.
+int enqueue_solve(hmpc_ctx* c, const hmpc::SolveIO& io, cudaStream_t st)
 {
-  if (B > c->max_batch) { g_err = "batch exceeds the context's capacity"; return HMPC_ERR_ARG; }
+  if (io.batch > c->max_batch) { g_err = "batch exceeds the context's capacity"; return HMPC_ERR_ARG; }
   CK(cudaSetDevice(c->device));
-  // per slot: [2 parities][8 words: list lengths of classes 0-2, wave-barrier counter, refinement list length, 3 unused],
-  // then the lists of class 1, class 2, the refinement class and class 0.  No classification kernel: the class-0 launch
-  // runs over every instance (or, in a masked call, over the list the selection kernel built from the mask) and hands the
-  // ones with more stance blocks than it holds to class 1's list.
-  // An eager chain uses the parity of its call count: the previous call's class-0 launch zeroed those lengths.  A graph
-  // replays the lengths it was recorded with and nothing zeroes them between replays, so a chain recorded into a graph
-  // uses the capture slot, starts with a memset node that zeroes both parities (the wave-barrier counter and the
-  // refinement list length included), and leaves the eager call count alone.
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   CK(cudaStreamIsCapturing(st, &cap));
   const bool capturing = cap != cudaStreamCaptureStatusNone;
-  if (capturing) slot = CAPTURE_SLOT;
-  int* base = c->d_cls + (size_t)slot * cls_slot_ints(c->max_batch);
-  const int par = capturing ? 0 : (c->tick[slot]++) & 1;
-  if (capturing) CK(cudaMemsetAsync(base, 0, 16 * sizeof(int), st));
-  int* counts = base + 8 * par;
-  int* counts_next = base + 8 * (par ^ 1);
-  // lists + i * max_batch is class i's list, i = 1, 2; i = 3: the refinement class's; i = 4: class 0's in a masked call
-  int* lists = base + 16 - (size_t)c->max_batch;
-  int* list0 = mask ? lists + (size_t)4 * c->max_batch : nullptr;
+  const int slot = capturing ? CAPTURE_SLOT : 0;
+  const hmpc::ClassSlot s{c->d_cls + (size_t)slot * hmpc::ClassSlot::cls_slot_ints(c->max_batch), c->max_batch,
+                          capturing ? 0 : (int)(c->tick[slot]++ & 1u)};
+  if (capturing) CK(cudaMemsetAsync(s.base, 0, hmpc::ClassSlot::HEAD_INTS * sizeof(int), st));
+  const hmpc::ChainLists lists = hmpc::slot_lists(s, io.mask != nullptr, c->cfg.refine);
   const bool pdl = pdl_enabled();
-  if (mask) {
+  if (io.mask) {
     // counts[0] of this parity was cleared by the previous call's class-0 launch: the kernel waits for it (griddepcontrol.wait)
     // before its first store, and class 0 reads the list after its own wait
-    CK(launch_chain(hmpc::hmpc_select_kernel<hmpc::SELECT_THREADS>, dim3(1), dim3(hmpc::SELECT_THREADS), 0, st, pdl, mask, B,
-                    list0, counts));
+    CK(launch_chain(hmpc::hmpc_select_kernel<hmpc::SELECT_THREADS>, dim3(1), dim3(hmpc::SELECT_THREADS), 0, st, pdl, io.mask,
+                    io.batch, s.list0(), s.counts()));
     CK(cudaGetLastError());
   }
-  for (int i = 0; i < c->ncls; i++) {
-    const ClassCfg& k = c->cls[i];
-    hmpc::KernelArgs ka = base_args(c, d_records, B, d_wrench32, d_status);
-    ka.wrench64 = d_wrench64;
-    ka.raw_records = reinterpret_cast<const unsigned char*>(raw);
-    ka.tau = d_tau;
-    ka.warm_start = (d_ws && ws_read) ? 1 : 0;
-    ka.ws_state = d_ws;
-    ka.ws_shift = ws_shift;
-    ka.ws_shifts = ws_shifts;
-    ka.list = (i == 0) ? list0 : lists + (size_t)i * c->max_batch;
-    ka.split_nb = (i == 0) ? k.nb_hi : -1;
-    ka.counts_next = (i == 0) ? counts_next : nullptr;
-    // arrival counter of class 0's wave barrier: the 4th length slot, which the chain does not use.  (Class 1 runs free:
-    // its instances differ more in length, and waiting for the slowest of every wave cost more than lockstep gained.)
-    ka.wave_sync = (c->lockstep && i == 0) ? reinterpret_cast<unsigned*>(counts + 3) : nullptr;
-    ka.counts = counts;
-    ka.cls = i;
-    ka.esc_list = (i + 1 < c->ncls) ? lists + (size_t)(i + 1) * c->max_batch : nullptr;
-    if (c->refine) {
-      ka.ref_list = lists + (size_t)3 * c->max_batch;
-      ka.ref_count = counts + 4;
-    }
-    ka.nb_cap = k.nb_cap;
-    ka.qmax = k.qmax;
-    ka.tcap = k.tcap;
-    ka.L = k.L;
-    ka.dbg_clk = g_dbg_clk;
-    const int grid = B < k.grid_cap ? B : k.grid_cap;
-    CK(launch_class(k, ka, grid, st, pdl));
-  }
-  if (c->refine) {
-    // the refinement class at the end of the chain: exits at once when nobody was handed over
-    hmpc::KernelArgs ka = refine_args(c, d_records, raw, B, d_wrench32, d_wrench64, d_status, d_tau, d_ws,
-                                      lists + (size_t)3 * c->max_batch, counts + 4);
-    ka.dbg_clk = g_dbg_clk;
-    const int grid = B < c->ref.grid_cap ? B : c->ref.grid_cap;
-    CK(launch_class(c->ref, ka, grid, st, pdl));
-  }
+  for (int i = 0; i < c->ncls; i++)
+    if (int rc = launch_class(c, i, io, lists, io.batch, st, pdl)) return rc;
+  // the refinement class at the end of the chain: exits at once when nobody was handed over
+  if (c->cfg.refine) return launch_class(c, hmpc::REFINE_CLASS, io, lists, io.batch, st, pdl);
   return HMPC_OK;
 }
 
-// the warm-started device-resident solve: robot i's proposal is its set in the context's d_ws, moved d_shift[i] steps
-// (d_shift NULL: every robot one step, the closed loop's tick); HMPC_WARM_START=0 makes it a cold solve
-int enqueue_solve_warm(hmpc_ctx* c, const void* d_records, int B, float* d_wrench, int* d_status, cudaStream_t st, float* d_tau,
-                       const int* d_shift, const unsigned char* d_mask = nullptr)
+// a device-resident call on device records and outputs.  warm: robot i's proposal is its set in the context's d_ws, moved
+// io.shifts[i] steps (NULL: every robot one step, the closed loop's tick); HMPC_WARM_START=0 makes it a cold solve
+hmpc::SolveIO device_call(const hmpc_ctx* c, const void* d_records, int B, float* d_wrench, int* d_status, float* d_tau, bool warm)
 {
-  return enqueue_solve(c, d_records, B, d_wrench, nullptr, d_status, st, 0, d_tau, c->warm_start ? c->d_ws : nullptr, 1, true,
-                       nullptr, d_shift, d_mask);
+  hmpc::SolveIO io;
+  io.records = d_records;
+  io.batch = B;
+  io.wrench = d_wrench;
+  io.status = d_status;
+  io.tau = d_tau;
+  if (warm && c->warm_start) io.ws = c->d_ws, io.warm = true;
+  return io;
 }
-}  // namespace
 
-namespace {
 // Host-buffer path: the host has the contact tables in hand while it packs, so it builds the class lists itself
-// (same rule as hmpc_classify_kernel) and launches only the non-empty classes — no classification kernel, no
-// empty launches.  Working-set overflow cannot escalate here; the caller re-runs such a chunk through enqueue_solve.
-// `mask` (the chunk's, host) or NULL: only the robots it lists go on the lists.
-void classify_host(const hmpc_ctx* c, const unsigned char* gait0, size_t gait_stride, int nb, int* blockbuf,
-                   const unsigned char* mask = nullptr)
+// (hmpc::classify_host) and launches only the non-empty classes — no classification kernel, no empty launches.
+// Working-set overflow cannot escalate here (enqueue_overflow_retry), nor can the refinement class run (enqueue_refine_retry).
+
+// the host-built lists of chunk `k` at `block` (device-readable) and the chunk's refinement list while refinement is on
+hmpc::ChainLists chunk_lists(const hmpc_ctx* c, int k, int* block, bool escalate)
 {
-  int* counts = blockbuf;
-  int* lists = blockbuf + 4;
-  counts[0] = counts[1] = counts[2] = counts[3] = 0;
-  const int N = c->horizon;
-  for (int i = 0; i < nb; i++) {
-    if (mask && !mask[i]) continue;
-    int k = 0;
-    for (int e = 0; e < 2 * N; e++) {
-      const float ub = c->setup.f_max * (float)gait0[(size_t)i * gait_stride + e];
-      k += !(ub < 0.0001f && ub > -0.0001f);
-    }
-    const int cl = (k <= c->cls[0].nb_hi) ? 0 : 1;
-    lists[(size_t)cl * c->max_batch + counts[cl]++] = i;
-  }
+  int* ref = c->d_ref + (size_t)k * (1 + (size_t)c->max_batch);
+  return hmpc::host_lists(block, c->max_batch, c->cfg.refine ? ref : nullptr, escalate);
 }
 
-int enqueue_solve_hostlists(hmpc_ctx* c, const void* d_records, int nb, int* h_block, float* d_wrench32, int* d_status,
-                            cudaStream_t st, int slot, float* d_tau, bool zero_copy, const update_data_t* raw = nullptr,
-                            double* wrench64 = nullptr, int* d_ws = nullptr, const int* ws_shifts = nullptr)
+int enqueue_solve_hostlists(hmpc_ctx* c, const hmpc::SolveIO& io, int* h_block, cudaStream_t st, int k, bool zero_copy)
 {
-  int* d_block = c->d_lists + (size_t)slot * (4 + 3 * (size_t)c->max_batch);
+  int* d_block = zero_copy ? h_block : c->d_lists + (size_t)k * hmpc::host_lists_ints(c->max_batch);
   const int n0 = h_block[0], n1 = h_block[1];
-  if (zero_copy) {
-    d_block = h_block;  // pinned + mapped: the kernels read the lists over PCIe, no copy launch
-  } else {
+  if (!zero_copy) {  // else pinned + mapped: the kernels read the lists over PCIe, no copy launch
     // counts + class-0 list (+ class-1 list when it is not empty) in one copy
-    const size_t ints = (n1 > 0) ? (size_t)4 + c->max_batch + n1 : (size_t)4 + n0;
+    const size_t ints = n1 > 0 ? hmpc::host_list(h_block, c->max_batch, 1) - h_block + n1 : hmpc::HOST_LIST_HEAD + n0;
     CK(cudaMemcpyAsync(d_block, h_block, ints * sizeof(int), cudaMemcpyHostToDevice, st));
   }
-  int* d_ref = c->d_ref + (size_t)slot * (1 + (size_t)c->max_batch);  // refinement list length + list of this chunk
-  if (c->refine) CK(cudaMemsetAsync(d_ref, 0, sizeof(int), st));
-  for (int i = 0; i < 2; i++) {
-    const int cnt = i == 0 ? n0 : n1;
-    if (cnt == 0) continue;
-    const ClassCfg& k = c->cls[i];
-    hmpc::KernelArgs ka = base_args(c, d_records, nb, d_wrench32, d_status);
-    ka.raw_records = reinterpret_cast<const unsigned char*>(raw);
-    ka.wrench64 = wrench64;
-    ka.tau = d_tau;
-    ka.warm_start = d_ws ? 1 : 0;
-    ka.ws_state = d_ws;
-    ka.ws_shift = 1;
-    ka.ws_shifts = ws_shifts;
-    ka.list = d_block + 4 + (size_t)i * c->max_batch;
-    ka.counts = d_block;
-    ka.cls = i;
-    ka.esc_list = nullptr;  // overflow is handled by the caller's retry
-    if (c->refine) {        // so is the refinement class (enqueue_refine_retry)
-      ka.ref_list = d_ref + 1;
-      ka.ref_count = d_ref;
-    }
-    ka.split_nb = -1;
-    ka.nb_cap = k.nb_cap;
-    ka.qmax = k.qmax;
-    ka.tcap = k.tcap;
-    ka.L = k.L;
-    ka.dbg_clk = g_dbg_clk;
-    const int grid = cnt < k.grid_cap ? cnt : k.grid_cap;
-    CK(launch_class(k, ka, grid, st));
-  }
+  const hmpc::ChainLists lists = chunk_lists(c, k, d_block, false);
+  if (c->cfg.refine) CK(cudaMemsetAsync(lists.ref_count, 0, sizeof(int), st));
+  for (int i = 0; i < 2; i++)
+    if (h_block[i] > 0)
+      if (int rc = launch_class(c, i, io, lists, h_block[i], st)) return rc;
   return HMPC_OK;
 }
 
@@ -883,52 +636,29 @@ int enqueue_solve_hostlists(hmpc_ctx* c, const void* d_records, int nb, int* h_b
 // instance that overflowed kept its proposal (the kernel does not record a set for it), so results, statuses and working
 // sets are those of the device-resident path.  `h_block` holds the chunk's class lists and is reused for the retry's.
 // `mask` (the chunk's, host) or NULL: the status words of robots it does not list are stale and are not looked at.
-int enqueue_overflow_retry(hmpc_ctx* c, const void* d_records, int nb, int* h_block, const int* h_status, float* d_wrench32,
-                           int* d_status, cudaStream_t st, int slot, float* d_tau, int* d_ws, const int* ws_shifts,
+int enqueue_overflow_retry(hmpc_ctx* c, const hmpc::SolveIO& io, int* h_block, const int* h_status, cudaStream_t st, int k,
                            const unsigned char* mask)
 {
-  const size_t mb = c->max_batch;
+  const int mb = c->max_batch, nb = io.batch;
   std::vector<char> was_cls1(nb, 0);
-  for (int j = 0; j < h_block[1]; j++) was_cls1[h_block[4 + mb + j]] = 1;
+  for (int j = 0; j < h_block[1]; j++) was_cls1[hmpc::host_list(h_block, mb, 1)[j]] = 1;
   int n[3] = {0, 0, 0};
   for (int i = 0; i < nb; i++) {
     if ((mask && !mask[i]) || HMPC_STATUS_CODE(h_status[i]) != hmpc::ST_WS_CAP) continue;
     const int next = was_cls1[i] ? 2 : 1;
-    if (next < c->ncls) h_block[4 + next * mb + n[next]++] = i;  // (class 1 as the last class: its overflow is final)
+    if (next < c->ncls) hmpc::host_list(h_block, mb, next)[n[next]++] = i;  // (class 1 as the last class: its overflow is final)
   }
   h_block[0] = 0;
   h_block[1] = n[1];
   h_block[2] = n[2];
   h_block[3] = 0;
-  int* d_block = c->d_lists + (size_t)slot * (4 + 3 * mb);
-  CK(cudaMemcpyAsync(d_block, h_block, (4 + 2 * mb + n[2]) * sizeof(int), cudaMemcpyHostToDevice, st));
+  int* d_block = c->d_lists + (size_t)k * hmpc::host_lists_ints(mb);
+  CK(cudaMemcpyAsync(d_block, h_block, (hmpc::host_list(h_block, mb, 2) - h_block + n[2]) * sizeof(int), cudaMemcpyHostToDevice, st));
+  const hmpc::ChainLists lists = chunk_lists(c, k, d_block, true);
   for (int i = 1; i < c->ncls; i++) {
     const int cnt = (i == 1) ? n[1] : n[1] + n[2];  // class 2's list grows by class 1's escalations
-    if (cnt == 0) continue;
-    const ClassCfg& k = c->cls[i];
-    hmpc::KernelArgs ka = base_args(c, d_records, nb, d_wrench32, d_status);
-    ka.tau = d_tau;
-    ka.warm_start = d_ws ? 1 : 0;
-    ka.ws_state = d_ws;
-    ka.ws_shift = 1;
-    ka.ws_shifts = ws_shifts;
-    ka.list = d_block + 4 + i * mb;
-    ka.counts = d_block;
-    ka.cls = i;
-    ka.esc_list = (i + 1 < c->ncls) ? d_block + 4 + (i + 1) * mb : nullptr;
-    if (c->refine) {
-      int* d_ref = c->d_ref + (size_t)slot * (1 + mb);
-      ka.ref_list = d_ref + 1;
-      ka.ref_count = d_ref;
-    }
-    ka.split_nb = -1;
-    ka.nb_cap = k.nb_cap;
-    ka.qmax = k.qmax;
-    ka.tcap = k.tcap;
-    ka.L = k.L;
-    ka.dbg_clk = g_dbg_clk;
-    const int grid = cnt < k.grid_cap ? cnt : k.grid_cap;
-    CK(launch_class(k, ka, grid, st));
+    if (cnt > 0)
+      if (int rc = launch_class(c, i, io, lists, cnt, st)) return rc;
   }
   return HMPC_OK;
 }
@@ -936,15 +666,10 @@ int enqueue_overflow_retry(hmpc_ctx* c, const void* d_records, int nb, int* h_bl
 // Refinement in a host-list launch: the kernels pushed the instances beyond the conditioning limit to the chunk's refinement
 // list (device memory), and the refinement class solves them as it does at the end of the device-resident chain.  Called
 // when refinement is on and a status of the chunk has code 4 (a non-positive pivot is not on the list).
-int enqueue_refine_retry(hmpc_ctx* c, const void* d_records, int nb, float* d_wrench32, int* d_status, cudaStream_t st, int slot,
-                         float* d_tau, int* d_ws)
+int enqueue_refine_retry(hmpc_ctx* c, const hmpc::SolveIO& io, cudaStream_t st, int k)
 {
-  int* d_ref = c->d_ref + (size_t)slot * (1 + (size_t)c->max_batch);
-  hmpc::KernelArgs ka = refine_args(c, d_records, nullptr, nb, d_wrench32, nullptr, d_status, d_tau, d_ws, d_ref + 1, d_ref);
-  ka.dbg_clk = g_dbg_clk;
-  const int grid = nb < c->ref.grid_cap ? nb : c->ref.grid_cap;
-  CK(launch_class(c->ref, ka, grid, st));
-  return HMPC_OK;
+  int* d_block = c->d_lists + (size_t)k * hmpc::host_lists_ints(c->max_batch);
+  return launch_class(c, hmpc::REFINE_CLASS, io, chunk_lists(c, k, d_block, false), io.batch, st);
 }
 }  // namespace
 
@@ -965,12 +690,12 @@ HMPC_EXTERNC void hmpc_debug_set_clock_buffer(long long* d_buf) { g_dbg_clk = d_
 namespace { int g_fail_next_solves = 0; }
 HMPC_EXTERNC void hmpc_debug_fail_next_solves(int n) { g_fail_next_solves = n; }
 
-HMPC_EXTERNC int hmpc_launches_per_solve(const hmpc_ctx* c) { return c ? c->ncls + (c->refine ? 1 : 0) : 0; }
+HMPC_EXTERNC int hmpc_launches_per_solve(const hmpc_ctx* c) { return c ? c->ncls + (c->cfg.refine ? 1 : 0) : 0; }
 
 HMPC_EXTERNC int hmpc_set_refinement(hmpc_ctx* c, int on)
 {
   if (!c) { g_err = "hmpc_set_refinement: null context"; return HMPC_ERR_ARG; }
-  c->refine = on ? 1 : 0;
+  c->cfg.refine = on ? 1 : 0;
   return HMPC_OK;
 }
 
@@ -991,7 +716,7 @@ HMPC_EXTERNC int hmpc_solve_device(hmpc_ctx* c, const void* d_records, int B, fl
   if (!c || !d_records || !d_wrench || !d_status || B < 0) { g_err = "hmpc_solve_device: bad argument"; return HMPC_ERR_ARG; }
   if (B == 0) return HMPC_OK;
   if (int rc = check_device_records(c, d_records, B, "hmpc_solve_device")) return rc;
-  return enqueue_solve(c, d_records, B, d_wrench, nullptr, d_status, static_cast<cudaStream_t>(stream));
+  return enqueue_solve(c, device_call(c, d_records, B, d_wrench, d_status, nullptr, false), static_cast<cudaStream_t>(stream));
 }
 
 HMPC_EXTERNC int hmpc_solve_device_ex(hmpc_ctx* c, const void* d_records, int B, float* d_wrench, int* d_status,
@@ -1000,7 +725,7 @@ HMPC_EXTERNC int hmpc_solve_device_ex(hmpc_ctx* c, const void* d_records, int B,
   if (!c || !d_records || !d_wrench || !d_status || B < 0) { g_err = "hmpc_solve_device_ex: bad argument"; return HMPC_ERR_ARG; }
   if (B == 0) return HMPC_OK;
   if (int rc = check_device_records(c, d_records, B, "hmpc_solve_device_ex")) return rc;
-  return enqueue_solve(c, d_records, B, d_wrench, nullptr, d_status, static_cast<cudaStream_t>(stream), 0, d_tau);
+  return enqueue_solve(c, device_call(c, d_records, B, d_wrench, d_status, d_tau, false), static_cast<cudaStream_t>(stream));
 }
 
 HMPC_EXTERNC int hmpc_solve_device_warm(hmpc_ctx* c, const void* d_records, int B, float* d_wrench, int* d_status, float* d_tau,
@@ -1009,7 +734,9 @@ HMPC_EXTERNC int hmpc_solve_device_warm(hmpc_ctx* c, const void* d_records, int 
   if (!c || !d_records || !d_wrench || !d_status || B < 0) { g_err = "hmpc_solve_device_warm: bad argument"; return HMPC_ERR_ARG; }
   if (B == 0) return HMPC_OK;
   if (int rc = check_device_records(c, d_records, B, "hmpc_solve_device_warm")) return rc;
-  return enqueue_solve_warm(c, d_records, B, d_wrench, d_status, static_cast<cudaStream_t>(stream), d_tau, d_shift);
+  hmpc::SolveIO io = device_call(c, d_records, B, d_wrench, d_status, d_tau, true);
+  io.shifts = d_shift;
+  return enqueue_solve(c, io, static_cast<cudaStream_t>(stream));
 }
 
 HMPC_EXTERNC int hmpc_solve_device_masked(hmpc_ctx* c, const void* d_records, int B, const unsigned char* d_mask, float* d_wrench,
@@ -1021,7 +748,10 @@ HMPC_EXTERNC int hmpc_solve_device_masked(hmpc_ctx* c, const void* d_records, in
   }
   if (B == 0) return HMPC_OK;
   if (int rc = check_device_records(c, d_records, B, "hmpc_solve_device_masked")) return rc;
-  return enqueue_solve_warm(c, d_records, B, d_wrench, d_status, static_cast<cudaStream_t>(stream), d_tau, d_shift, d_mask);
+  hmpc::SolveIO io = device_call(c, d_records, B, d_wrench, d_status, d_tau, true);
+  io.shifts = d_shift;
+  io.mask = d_mask;
+  return enqueue_solve(c, io, static_cast<cudaStream_t>(stream));
 }
 
 HMPC_EXTERNC int hmpc_assemble_device(hmpc_ctx* c, const void* d_records, int B, float* d_H, float* d_g,
@@ -1034,25 +764,16 @@ HMPC_EXTERNC int hmpc_assemble_device(hmpc_ctx* c, const void* d_records, int B,
   if (B == 0) return HMPC_OK;
   if (int rc = check_device_records(c, d_records, B, "hmpc_assemble_device")) return rc;
   CK(cudaSetDevice(c->device));
-  const ClassCfg& k = c->cls[c->ncls - 1];
-  hmpc::KernelArgs ka = base_args(c, d_records, B, nullptr, c->d_status);
-  ka.list = nullptr;  // identity
-  ka.split_nb = -1;
-  ka.counts = c->d_counts;
-  ka.cls = c->ncls - 1;
-  ka.esc_list = nullptr;
-  ka.nb_cap = k.nb_cap;
-  ka.qmax = k.qmax;
-  ka.tcap = k.tcap;
-  ka.L = k.L;
-  ka.dbg_H = d_H;
-  ka.dbg_g = d_g;
-  ka.dbg_F = d_Fblk;
-  ka.dbg_lb = d_lb;
-  ka.dbg_ub = d_ub;
-  const int grid = B < k.grid_cap ? B : k.grid_cap;
-  CK(launch_class(k, ka, grid, static_cast<cudaStream_t>(stream)));
-  return HMPC_OK;
+  // the last class over every robot (no list), dumping its QP data
+  hmpc::SolveIO io = device_call(c, d_records, B, nullptr, c->d_status, nullptr, false);
+  io.dump_H = d_H;
+  io.dump_g = d_g;
+  io.dump_F = d_Fblk;
+  io.dump_lb = d_lb;
+  io.dump_ub = d_ub;
+  hmpc::ChainLists lists;
+  lists.counts = c->d_counts;
+  return launch_class(c, c->ncls - 1, io, lists, B, static_cast<cudaStream_t>(stream));
 }
 
 static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_state_t* sin, int B, double* wrench_out,
@@ -1184,7 +905,7 @@ HMPC_EXTERNC int hmpc_rollout_device(hmpc_ctx* c, hmpc_state_t* d_states, hmpc_r
     if (d_record_log)
       CK(cudaMemcpyAsync(static_cast<unsigned char*>(d_record_log) + (size_t)t * B * c->rec_stride, c->d_rec,
                          (size_t)B * c->rec_stride, cudaMemcpyDeviceToDevice, st));
-    rc = enqueue_solve_warm(c, c->d_rec, B, dw, ds, st, nullptr, nullptr);
+    rc = enqueue_solve(c, device_call(c, c->d_rec, B, dw, ds, nullptr, true), st);
     if (rc != HMPC_OK) return rc;
     hmpc::hmpc_advance_kernel<<<(B + 63) / 64, 64, 0, st>>>(reinterpret_cast<unsigned char*>(d_states),
                                                             reinterpret_cast<unsigned char*>(d_loop), B, c->horizon, dtMPC, dw, ds,
@@ -1276,8 +997,18 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
     int* ds = status ? status : reinterpret_cast<int*>(c->h_out + (size_t)c->max_batch * nw * 4);
     float* dt_ = tau_out ? reinterpret_cast<float*>(c->h_out + (size_t)c->max_batch * (nw * 4 + 4)) : nullptr;
     if (mask) memcpy(c->h_mask, mask, (size_t)B);  // pinned: the selection kernel reads it mapped
-    int rc = enqueue_solve(c, nullptr, B, c->shard_out, wrench_out, ds, c->stream, 0, dt_, ws, 1, ws != nullptr, in, hsh,
-                           mask ? c->h_mask : nullptr);
+    hmpc::SolveIO io;
+    io.raw = in;
+    io.batch = B;
+    io.wrench = c->shard_out;
+    io.wrench64 = wrench_out;
+    io.status = ds;
+    io.tau = dt_;
+    io.ws = ws;
+    io.warm = ws != nullptr;
+    io.shifts = hsh;
+    io.mask = mask ? c->h_mask : nullptr;
+    int rc = enqueue_solve(c, io, c->stream);
     if (rc != HMPC_OK) return rc;
     if (c->shard_out) {
       CK(cudaEventRecord(c->solved, c->stream));
@@ -1301,6 +1032,8 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
   int lo[NCHUNK + 1];
   for (int k = 0; k <= nch; k++) lo[k] = (int)((long long)B * k / nch);
   cudaStream_t sts[NCHUNK] = {c->stream, c->xstream[0], c->xstream[1], c->xstream[2]};
+  hmpc::SolveIO io[NCHUNK];  // each chunk's device views of records, results, working sets and shifts
+  int* hblk[NCHUNK];         // and its host-built lists
   for (int k = 0; k < nch; k++) {
     const int b0 = lo[k], nb = lo[k + 1] - lo[k];
     if (nb == 0) continue;
@@ -1338,23 +1071,25 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
     }
     const size_t ooff = (size_t)b0 * (nw * 4 + 4 + 40), obytes = (size_t)nb * (nw * 4 + 4 + (tau_out ? 40 : 0));
     unsigned char* obase = zc ? c->h_out : c->d_out;
-    float* dw = reinterpret_cast<float*>(obase + ooff);
-    int* ds = reinterpret_cast<int*>(obase + ooff + (size_t)nb * nw * 4);
-    float* dt_ = tau_out ? reinterpret_cast<float*>(obase + ooff + (size_t)nb * (nw * 4 + 4)) : nullptr;
-    const unsigned char* rbase = (zc && !sin) ? c->h_rec : c->d_rec;
-    int* hblk = c->h_cls + (size_t)k * (4 + 3 * (size_t)c->max_batch);
-    if (sin) classify_host(c, sin[b0].gait, sizeof(hmpc_state_t), nb, hblk);
-    else classify_host(c, in[b0].gait, sizeof(update_data_t), nb, hblk, mask ? mask + b0 : nullptr);
-    int* ws_k = ws ? ws + (size_t)b0 * hmpc::WS_STATE_INTS : nullptr;
-    const int* sh_k = nullptr;
+    io[k].records = ((zc && !sin) ? c->h_rec : c->d_rec) + (size_t)b0 * c->rec_stride;
+    io[k].batch = nb;
+    io[k].wrench = reinterpret_cast<float*>(obase + ooff);
+    io[k].status = reinterpret_cast<int*>(obase + ooff + (size_t)nb * nw * 4);
+    io[k].tau = tau_out ? reinterpret_cast<float*>(obase + ooff + (size_t)nb * (nw * 4 + 4)) : nullptr;
+    io[k].ws = ws ? ws + (size_t)b0 * hmpc::WS_STATE_INTS : nullptr;
+    io[k].warm = ws != nullptr;
     if (hsh && zc) {
-      sh_k = hsh + b0;  // mapped, like the records and lists of this mode
+      io[k].shifts = hsh + b0;  // mapped, like the records and lists of this mode
     } else if (hsh) {
       CK(cudaMemcpyAsync(c->d_shift + b0, hsh + b0, (size_t)nb * sizeof(int), cudaMemcpyHostToDevice, sts[k]));
-      sh_k = c->d_shift + b0;
+      io[k].shifts = c->d_shift + b0;
     }
-    rc = enqueue_solve_hostlists(c, rbase + (size_t)b0 * c->rec_stride, nb, hblk, dw, ds, sts[k], k, dt_, zc, nullptr, nullptr,
-                                 ws_k, sh_k);
+    hblk[k] = c->h_cls + (size_t)k * hmpc::host_lists_ints(c->max_batch);
+    if (sin) hmpc::classify_host(c->horizon, c->cfg.f_max, c->cls[0].nb_hi, sin[b0].gait, sizeof(hmpc_state_t), nb, hblk[k], c->max_batch);
+    else
+      hmpc::classify_host(c->horizon, c->cfg.f_max, c->cls[0].nb_hi, in[b0].gait, sizeof(update_data_t), nb, hblk[k], c->max_batch,
+                          mask ? mask + b0 : nullptr);
+    rc = enqueue_solve_hostlists(c, io[k], hblk[k], sts[k], k, zc);
     if (rc != HMPC_OK) return rc;
     if (!zc) CK(cudaMemcpyAsync(c->h_out + ooff, c->d_out + ooff, obytes, cudaMemcpyDeviceToHost, sts[k]));
     if (trace) tr[ntr++] = now();
@@ -1371,21 +1106,10 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
       bool overflow = false, not_spd = false;
       for (int i = 0; i < nb; i++) overflow |= listed(b0 + i) && (HMPC_STATUS_CODE(hs[i]) == hmpc::ST_WS_CAP);
       for (int i = 0; i < nb; i++) not_spd |= listed(b0 + i) && (HMPC_STATUS_CODE(hs[i]) == hmpc::ST_NOT_SPD);
-      const bool refine = c->refine && not_spd;  // instances handed to the refinement class (on its device-side list)
+      const bool refine = c->cfg.refine && not_spd;  // instances handed to the refinement class (on its device-side list)
       if (overflow || refine) {
-        unsigned char* obase = zc ? c->h_out : c->d_out;
-        float* dw = reinterpret_cast<float*>(obase + ooff);
-        int* ds = reinterpret_cast<int*>(obase + ooff + (size_t)nb * nw * 4);
-        float* dt_ = tau_out ? reinterpret_cast<float*>(obase + ooff + (size_t)nb * (nw * 4 + 4)) : nullptr;
-        const unsigned char* rbase = (zc && !sin) ? c->h_rec : c->d_rec;
-        int* hblk = c->h_cls + (size_t)k * (4 + 3 * (size_t)c->max_batch);
-        const int* sh_k = hsh ? (zc ? hsh : c->d_shift) + b0 : nullptr;  // where the first pass read them
-        int* ws_k = ws ? ws + (size_t)b0 * hmpc::WS_STATE_INTS : nullptr;
-        int rc = overflow ? enqueue_overflow_retry(c, rbase + (size_t)b0 * c->rec_stride, nb, hblk, hs, dw, ds, sts[k], k, dt_,
-                                                   ws_k, sh_k, mask ? mask + b0 : nullptr)
-                          : HMPC_OK;
-        if (rc == HMPC_OK && refine)
-          rc = enqueue_refine_retry(c, rbase + (size_t)b0 * c->rec_stride, nb, dw, ds, sts[k], k, dt_, ws_k);
+        int rc = overflow ? enqueue_overflow_retry(c, io[k], hblk[k], hs, sts[k], k, mask ? mask + b0 : nullptr) : HMPC_OK;
+        if (rc == HMPC_OK && refine) rc = enqueue_refine_retry(c, io[k], sts[k], k);
         if (rc != HMPC_OK) return rc;
         if (!zc)
           CK(cudaMemcpyAsync(c->h_out + ooff, c->d_out + ooff, (size_t)nb * (nw * 4 + 4 + (tau_out ? 40 : 0)),
@@ -1496,7 +1220,7 @@ HMPC_EXTERNC void setup_problem(double dt, int horizon, double mu, double f_max)
   s.horizon = horizon;
   // the reference's caller sets the same problem up before every tick; a different QP (dt, f_max) forgets the warm start's
   // working set (a new context — another horizon — starts without one)
-  if (s.dt != g_ctx->setup.dt || s.f_max != g_ctx->setup.f_max)
+  if (s.dt != g_ctx->cfg.dt || s.f_max != g_ctx->cfg.f_max)
     if (hmpc_reset_warm_start(g_ctx, g_ctx->stream) != HMPC_OK) die("setup_problem");
   hmpc_set_problem(g_ctx, &s);
 }

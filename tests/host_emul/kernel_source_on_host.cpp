@@ -5,11 +5,12 @@
 //     — one call per robot with threadIdx/blockIdx set the way a launch would set them;
 //   * the stage-1 device functions of the solve kernel (role_leg / role_state / role_inertia: SRBD linearisation, foot
 //     rotations, constraint rows) and the joint-torque epilogue function (leg_torque, f-2).
-//   * the classification kernel and the solve kernel itself (all stages), one OS thread per CUDA thread of one CTA at a
-//     time, launched the way hmpc_capi.cu's enqueue_solve launches them (classification -> class 0 -> class 1 -> class 2
-//     with working-set-overflow escalation through the lists)
-// so that tests/test_kernel_source_on_host.py can hold the kernels' SOURCE to the oracle / to the reference's compiled
-// controller without a GPU.
+//   * the selection kernel and the solve kernel itself (all stages), one OS thread per CUDA thread of one CTA at a time,
+//     in the launch sequences of hmpc_capi.cu (emul_solve).  The kernel variants, the class shapes, the class-list memory
+//     and every launch's arguments come from the library's own hmpc_chain.h.
+// so that the CPU suite (tests/test_kernel_source_on_host.py, test_warm_start_calls.py, test_masked_solve.py,
+// test_refinement.py) can hold the kernels' SOURCE to the oracle / to the reference's compiled controller without a GPU.
+// race_driver.cpp makes the same source a command-line program for ThreadSanitizer.
 #include <cstdlib>
 #include <cstring>
 #include <thread>
@@ -24,6 +25,7 @@
 //   - every other `asm volatile(...)` (fences, griddepcontrol: no arithmetic) -> nothing
 // Everything else is the product's source, byte for byte.
 #include HMPC_DEVICE_HEADER
+#include "../../hector_simulation_b200/csrc/hmpc_chain.h"
 
 thread_local hmpc_emul_dim3 threadIdx, blockIdx, blockDim, gridDim;
 thread_local hmpc_emul::Cta* hmpc_emul_cta = nullptr;
@@ -60,61 +62,35 @@ void run_cta(int NT, F fn)
   delete cta;
 }
 
-// the kernel variants of hmpc_capi.cu (HMPC_FOR_VARIANT): <threads, min CTAs/SM, fixed horizon, class>
-const int kBucketThreads[5] = {64, 128, 192, 256, 384};
-int variant_threads(int variant) { return variant == 0 ? 128 : (variant == 1 ? 256 : kBucketThreads[(variant - 10) % 5]); }
-void launch_variant(int variant, const hmpc::KernelArgs& ka)
+// hmpc_capi.cu's launch of class `cls`: its arguments (hmpc::launch_args), and one emulated CTA that walks every instance
+// of the class
+void run_class(const hmpc::SolverSettings& S, int N, int ncls, int cls, const hmpc::ClassCfg& k, const hmpc::SolveIO& io,
+               const hmpc::ChainLists& lists)
 {
-  switch (variant) {
-    case 0: run_cta(128, [=] { hmpc::hmpc_solve_kernel<128, 7, 10, 0>(ka); }); break;
-    case 1: run_cta(256, [=] { hmpc::hmpc_solve_kernel<256, 2, 10, 1>(ka); }); break;
-    case 10: run_cta(64, [=] { hmpc::hmpc_solve_kernel<64, 8, 0, 0>(ka); }); break;
-    case 11: run_cta(128, [=] { hmpc::hmpc_solve_kernel<128, 6, 0, 0>(ka); }); break;
-    case 12: run_cta(192, [=] { hmpc::hmpc_solve_kernel<192, 3, 0, 0>(ka); }); break;
-    case 13: run_cta(256, [=] { hmpc::hmpc_solve_kernel<256, 2, 0, 0>(ka); }); break;
-    case 14: run_cta(384, [=] { hmpc::hmpc_solve_kernel<384, 1, 0, 0>(ka); }); break;
-    case 15: run_cta(64, [=] { hmpc::hmpc_solve_kernel<64, 8, 0, 1>(ka); }); break;
-    case 16: run_cta(128, [=] { hmpc::hmpc_solve_kernel<128, 6, 0, 1>(ka); }); break;
-    case 17: run_cta(192, [=] { hmpc::hmpc_solve_kernel<192, 3, 0, 1>(ka); }); break;
-    case 18: run_cta(256, [=] { hmpc::hmpc_solve_kernel<256, 2, 0, 1>(ka); }); break;
-    default: run_cta(384, [=] { hmpc::hmpc_solve_kernel<384, 1, 0, 1>(ka); }); break;
+  const hmpc::KernelArgs ka = hmpc::launch_args(S, N, ncls, cls, k, io, lists);
+  switch (k.variant) {
+#define HMPC_RUN(ID, NT, MB, NF, CL) \
+  case ID: run_cta(NT, [=] { hmpc::hmpc_solve_kernel<NT, MB, NF, CL>(ka); }); return;
+    HMPC_VARIANTS(HMPC_RUN)
+#undef HMPC_RUN
   }
+  hmpc_emul::die("no such kernel variant");
 }
-struct ClassCfg {
-  int variant, nb_cap, qmax, tcap;
-  hmpc::Layout L;
-};
-// hmpc_capi.cu build_classes, minus the CUDA occupancy calls
-int build_classes(int N, ClassCfg* cls)
+void run_select(const unsigned char* mask, int B, int* list, int* count)
 {
-  const int rs = hmpc::record_stride(N);
-  int ncls = 3;
-  for (int i = 0; i < 2; i++) {
-    ClassCfg& k = cls[i];
-    k.nb_cap = hmpc::class_nb_cap(N, i);
-    const int warps = hmpc::class_warps(N, i);
-    int bucket = 0;
-    while (bucket < 4 && kBucketThreads[bucket] < 32 * warps) bucket++;
-    k.variant = (N == 10) ? i : 10 + 5 * i + bucket;
-    k.qmax = hmpc::class_qmax(N, i);
-    k.tcap = hmpc::class_tcap(N, i);
-    k.L = hmpc::make_layout(N, k.nb_cap, k.qmax, rs, variant_threads(k.variant) / 32, k.tcap);
-  }
-  {
-    ClassCfg& k = cls[2];
-    k = cls[1];
-    if (N == 10) k.variant = 18;
-    const int n = 6 * k.nb_cap, nw = variant_threads(k.variant) / 32;
-    k.qmax = n;
-    k.tcap = 0;
-    k.L = hmpc::make_layout(N, k.nb_cap, k.qmax, rs, nw, 0);
-    while (k.L.total > 226 * 1024 && k.qmax > cls[1].qmax) {
-      k.qmax -= 4;
-      k.L = hmpc::make_layout(N, k.nb_cap, k.qmax, rs, nw, 0);
-    }
-    if (k.qmax <= cls[1].qmax || cls[1].qmax >= n) ncls = 2;
-  }
-  return ncls;
+  run_cta(hmpc::SELECT_THREADS, [=] { hmpc::hmpc_select_kernel<hmpc::SELECT_THREADS>(mask, B, list, count); });
+}
+// hmpc_create's settings, read per call: the same environment overrides, plus the two tolerances (the tolerance-sweep test)
+hmpc::SolverSettings settings(int refine)
+{
+  hmpc::SolverSettings S;
+  if (const char* e = getenv("HMPC_TOL_KKT")) S.tol_kkt = atof(e);
+  if (const char* e = getenv("HMPC_TOL_DEP")) S.tol_dep = atof(e);
+  if (const char* e = getenv("HMPC_KAPPA_MAX")) S.kappa_max = atof(e);
+  if (const char* e = getenv("HMPC_BLOCK_MIN")) S.block_min = atoi(e);
+  if (const char* e = getenv("HMPC_BLOCK_ROUNDS")) S.block_rounds = atoi(e);
+  S.refine = refine;
+  return S;
 }
 const unsigned kBlock = 128;
 inline void set_thread(int i)
@@ -126,21 +102,10 @@ inline void set_thread(int i)
 }
 }  // namespace
 
-namespace {
-int* g_ws = nullptr;  // [B][WS_STATE_INTS] working sets kept between emul_solve* calls (closed-loop warm start), or null
-int g_ws_shift = 0;
-}  // namespace
-
 extern "C" {
 
-/* working-set memory for the following emul_solve* calls: written back by every solve, proposed to the next one when that
- * call passes warm_start = 1 (shift = MPC steps the horizon moved in between) */
-void emul_set_ws(int* ws, int shift)
-{
-  g_ws = ws;
-  g_ws_shift = shift;
-}
 int emul_ws_ints() { return hmpc::WS_STATE_INTS; }
+int emul_select_threads() { return hmpc::SELECT_THREADS; }
 
 int emul_record_stride(int N) { return hmpc::record_stride(N); }
 
@@ -190,93 +155,87 @@ void emul_stage1(const float* rf, float dt, float* Fblk, float* x0, float* Acd, 
   memcpy(x0, x0f, 13 * sizeof(float));
 }
 
-/* The solve paths of hmpc_capi.cu on B <= 1024 robots.
- *   records != NULL: the device-resident path (enqueue_solve): classification kernel, then one launch per size class with
- *                    escalation lists, reading packed records.
- *   raw != NULL    : the in-place host-buffer path (enqueue_solve_hostlists): class lists built on the host from the contact
- *                    tables, kernels gather the live bytes of the caller's update_data_t records (3016-byte stride), no
- *                    escalation (the caller retries overflow through the first path).
- * Outputs: wrench [B][12N] floats and/or wrench64 [B][12N] doubles, status [B], tau [B][10] or NULL, launched[3] =
- * instances each class processed (NULL to skip).  warm_start: KernelArgs::warm_start.  Optional assembly dump (all NULL,
- * or all given): H [B][n*n], g [B][n], Fblk [B][192], lb/ub [B][16N]. */
-int emul_solve_ex(const unsigned char* records, const unsigned char* raw, int B, int N, float dt, float f_max, int max_iter,
-                  int warm_start, float* wrench, double* wrench64, int* status, float* tau, int* launched, float* dH, float* dg,
-                  float* dF, float* dlb, float* dub)
+/* the selection kernel of a masked call on one emulated CTA: list[0 .. *count) = the robots i < B with mask[i] != 0 */
+void emul_select(const unsigned char* mask, int B, int* list, int* count) { run_select(mask, B, list, count); }
+
+/* the class shapes of horizon N (hmpc::plan_classes): out[4][6] = variant, threads, shared-memory bytes, working-set
+ * capacity, blocks of 6 variables, cached columns of classes 0-2 and the refinement class; returns the number of classes */
+int emul_plan(int N, int* out)
 {
-  if (B < 1 || B > 1024 || (!records && !raw)) return 1;
-  ClassCfg cls[3];
-  int ncls = build_classes(N, cls);
-  std::vector<int> block(8 + 3 * (size_t)B, 0);
-  int* counts = block.data();      // [4] list lengths (+ [4] the next call's, which the class-0 launch clears)
-  int* lists = counts + 8;
-  const int rs = hmpc::record_stride(N);
-  const int nb_hi0 = cls[0].nb_cap;
-  if (raw) {
-    // hmpc_capi.cu classify_host: gait bytes at offsetof(update_data_t, gait) = 1944
-    for (int i = 0; i < B; i++) {
-      int k = 0;
-      for (int e = 0; e < 2 * N; e++) {
-        const float ub = f_max * (float)raw[(size_t)i * 3016 + 1944 + e];
-        k += !(ub < 0.0001f && ub > -0.0001f);
-      }
-      const int cl = (k <= nb_hi0) ? 0 : 1;
-      lists[(size_t)cl * B + counts[cl]++] = i;
-    }
-    ncls = 2;
-  } else {
-    counts[0] = B;       // device-resident path: class 0 runs over every instance and classifies on the way
-    counts[4] = counts[5] = counts[6] = counts[7] = 0x55;  // must come back cleared
+  hmpc::ClassCfg cls[3], ref;
+  const int ncls = hmpc::plan_classes(N, cls, ref);
+  for (int i = 0; i < 4; i++) {
+    const hmpc::ClassCfg& k = i < 3 ? cls[i] : ref;
+    const int row[6] = {k.variant, k.threads, k.smem, k.qmax, k.nb_cap, k.tcap};
+    memcpy(out + 6 * i, row, sizeof row);
   }
-  for (int i = 0; i < ncls; i++) {
-    if (launched) launched[i] = counts[i];
-    if (counts[i] == 0) continue;
-    const bool fused = !raw && i == 0;
-    hmpc::KernelArgs ka{};
-    ka.records = records;
-    ka.raw_records = raw;
-    ka.rec_stride = rs;
-    ka.batch = B;
-    ka.horizon = N;
-    ka.dt = dt;
-    ka.f_max = f_max;
-    ka.max_iter = max_iter;
-    ka.tol_kkt = getenv("HMPC_TOL_KKT") ? atof(getenv("HMPC_TOL_KKT")) : 1e-9;   // hmpc_capi.cu's constants; the
-    ka.tol_dep = getenv("HMPC_TOL_DEP") ? atof(getenv("HMPC_TOL_DEP")) : 1e-11;  // tolerance-sweep test overrides them
-    ka.kappa_max = getenv("HMPC_KAPPA_MAX") ? atof(getenv("HMPC_KAPPA_MAX")) : 1.5e5;  // hmpc_capi.cu's default
-    ka.block_min = getenv("HMPC_BLOCK_MIN") ? atoi(getenv("HMPC_BLOCK_MIN")) : 2;  // hmpc_capi.cu's default
-    ka.block_rounds = getenv("HMPC_BLOCK_ROUNDS") ? atoi(getenv("HMPC_BLOCK_ROUNDS")) : 4;  // hmpc_capi.cu's default
-    ka.wrench = wrench;
-    ka.wrench64 = wrench64;
-    ka.status = status;
-    ka.tau = tau;
-    ka.warm_start = (g_ws && warm_start) ? 1 : 0;
-    ka.ws_state = g_ws;
-    ka.ws_shift = g_ws_shift;
-    ka.list = fused ? nullptr : lists + (size_t)i * B;
-    ka.split_nb = fused ? nb_hi0 : -1;
-    ka.counts_next = fused ? counts + 4 : nullptr;
-    ka.wave_sync = fused ? reinterpret_cast<unsigned*>(counts + 3) : nullptr;  // one emulated CTA walks all instances: B waves
-    ka.counts = counts;
-    ka.cls = i;
-    ka.esc_list = (!raw && i + 1 < ncls) ? lists + (size_t)(i + 1) * B : nullptr;
-    ka.nb_cap = cls[i].nb_cap;
-    ka.qmax = cls[i].qmax;
-    ka.tcap = cls[i].tcap;
-    ka.L = cls[i].L;
-    ka.dbg_H = dH; ka.dbg_g = dg; ka.dbg_F = dF; ka.dbg_lb = dlb; ka.dbg_ub = dub;
-    launch_variant(cls[i].variant, ka);
-    if (fused) {
-      if (counts[4] | counts[5] | counts[6] | counts[7]) return 2;  // the next call's lengths were not cleared
-      if (launched) launched[0] = B - counts[1];                     // instances class 0 kept
-    }
-  }
-  return 0;
+  return ncls;
 }
 
-int emul_solve(const unsigned char* records, int B, int N, float dt, float f_max, int max_iter, float* wrench, int* status,
-               float* tau, int* launched, float* dH, float* dg, float* dF, float* dlb, float* dub)
+/* One solve call of hmpc_capi.cu on B <= 1024 robots, each class on one emulated CTA.
+ *   hostlists == 0: enqueue_solve's device-resident chain over packed `records` or, in place, the caller's update_data_t
+ *                   records `raw` (the in-place mode): [the selection kernel over `mask`] -> class 0 over every robot (or the
+ *                   listed ones), classifying on the way -> class 1 -> class 2 through the escalation lists -> [refinement].
+ *   hostlists != 0: enqueue_solve_hostlists's launches over packed `records` (the zero-copy and copy-pipeline modes): class
+ *                   lists built on the host from the contact tables, no escalation; with refinement on, then
+ *                   enqueue_refine_retry's launch over the instances handed over.
+ * refine: hmpc_set_refinement.  ws [B][WS_STATE_INTS] working sets, written back (proposed when warm != 0, moved `shift`
+ * steps, or shifts[i] when shifts is not NULL), or NULL.  Outputs: wrench [B][12N] floats and/or wrench64 doubles, status [B],
+ * tau [B][10] or NULL, launched[4] = instances class 0 kept, class 1, class 2 and the refinement class took (NULL to skip).
+ * Optional assembly dump (all NULL, or all given): H [B][n*n], g [B][n], Fblk [B][192], lb/ub [B][16N].
+ * Returns 2 when class 0 did not clear the next call's length words. */
+int emul_solve(const unsigned char* records, const unsigned char* raw, int B, int N, int hostlists, int refine,
+               const unsigned char* mask, int* ws, int warm, int shift, const int* shifts, float* wrench, double* wrench64,
+               int* status, float* tau, int* launched, float* dH, float* dg, float* dF, float* dlb, float* dub)
 {
-  return emul_solve_ex(records, nullptr, B, N, dt, f_max, max_iter, 0, wrench, nullptr, status, tau, launched, dH, dg, dF, dlb, dub);
+  if (B < 1 || B > 1024 || (!records && !raw) || (hostlists && !records)) return 1;
+  const hmpc::SolverSettings S = settings(refine);
+  hmpc::ClassCfg cls[3], ref;
+  const int ncls = hmpc::plan_classes(N, cls, ref);
+  if (ncls == 0) return 1;
+  hmpc::SolveIO io;
+  io.records = records;
+  io.raw = raw;
+  io.batch = B;
+  io.wrench = wrench;
+  io.wrench64 = wrench64;
+  io.status = status;
+  io.tau = tau;
+  io.ws = ws;
+  io.warm = warm != 0;
+  io.shift = shift;
+  io.shifts = shifts;
+  io.mask = mask;
+  io.dump_H = dH, io.dump_g = dg, io.dump_F = dF, io.dump_lb = dlb, io.dump_ub = dub;
+  int la[4] = {0, 0, 0, 0};
+  std::vector<int> mem;
+  hmpc::ChainLists lists;
+  if (!hostlists) {
+    mem.assign(hmpc::ClassSlot::cls_slot_ints(B), 0);
+    const hmpc::ClassSlot slot{mem.data(), B, 0};
+    int* next = slot.counts_next();
+    for (int w = 0; w < 5; w++) next[w] = 0x55;  // the class-0 launch must clear them
+    lists = hmpc::slot_lists(slot, mask != nullptr, S.refine);
+    if (mask) run_select(mask, B, slot.list0(), slot.counts());
+    for (int i = 0; i < ncls; i++) {
+      const int n = (i == 0 && !mask) ? B : lists.counts[i];
+      if (n == 0) continue;
+      run_class(S, N, ncls, i, cls[i], io, lists);
+      la[i] = i == 0 ? n - lists.counts[1] : n;  // class 0 hands instances to class 1 as it classifies or overflows
+      if (i == 0 && (next[0] | next[1] | next[2] | next[3] | next[4])) return 2;
+    }
+  } else {
+    mem.assign(hmpc::host_lists_ints(B) + 1 + B, 0);
+    int* block = mem.data();
+    int* ref_list = block + hmpc::host_lists_ints(B);  // [length | entries], as hmpc_ctx::d_ref
+    hmpc::classify_host(N, S.f_max, cls[0].nb_hi, records + (54 + 12 * N) * 4, hmpc::record_stride(N), B, block, B, mask);
+    lists = hmpc::host_lists(block, B, S.refine ? ref_list : nullptr, false);
+    for (int i = 0; i < 2; i++)
+      if ((la[i] = block[i]) > 0) run_class(S, N, ncls, i, cls[i], io, lists);
+  }
+  if (S.refine && (la[3] = *lists.ref_count) > 0) run_class(S, N, ncls, hmpc::REFINE_CLASS, ref, io, lists);
+  if (launched) memcpy(launched, la, sizeof la);
+  return 0;
 }
 
 /* the torque epilogue's per-joint function: tau_j = column j of J_force_moment(q5, leg) . f6 */

@@ -84,26 +84,72 @@ def _host_buildable(src: str) -> str:
     return src
 
 
+_BUILT = {}
+
+
+def _compile(name, flags, tail=()):
+    """g++ on tests/host_emul/kernel_source_on_host.cpp with the host-buildable device header, written once per process"""
+    hdr = os.path.join(BUILD, "hmpc_device_host.cuh")
+    if "header" not in _BUILT:
+        os.makedirs(BUILD, exist_ok=True)
+        with open(hdr, "w") as f:
+            f.write(_host_buildable(open(DEVICE_HEADER).read()))
+        _BUILT["header"] = hdr
+    out = os.path.join(BUILD, name)
+    cmd = ["g++", "-std=c++17", "-ffp-contract=off", "-w", "-pthread", *flags,
+           "-I" + os.path.join(HERE, "fake_cuda"), "-I" + os.path.join(ROOT, "include"),
+           '-DHMPC_DEVICE_HEADER="%s"' % hdr, os.path.join(HERE, "kernel_source_on_host.cpp"), *tail, "-o", out]
+    return out, subprocess.run(cmd, capture_output=True, text=True)
+
+
+def host_emulation():
+    """The kernel source built for the host as a library (kernel_source_on_host.cpp), once per process: every test module
+    that runs the kernels on the host loads this one."""
+    if "lib" not in _BUILT:
+        lib, r = _compile("libkernel_source_on_host.so", ["-O2", "-fPIC", "-shared"], ["-l:libstdc++.so.6"])
+        assert r.returncode == 0, r.stderr[-3000:]
+        L = ctypes.CDLL(lib)
+        L.emul_leg_torque.restype = ctypes.c_double
+        _BUILT["lib"] = L
+    return _BUILT["lib"]
+
+
+def race_driver():
+    """The ThreadSanitizer build of the kernel source with race_driver.cpp's main, once per process; skips the calling test
+    when the toolchain has no ThreadSanitizer runtime."""
+    if "race" not in _BUILT:
+        exe, r = _compile("race_driver_tsan", ["-O1", "-g", "-fsanitize=thread"], [os.path.join(HERE, "race_driver.cpp")])
+        _BUILT["race"] = (exe, r.returncode, r.stderr[-300:])
+    exe, rc, err = _BUILT["race"]
+    if rc != 0:
+        pytest.skip("no ThreadSanitizer runtime with this toolchain: " + err)
+    return exe
+
+
 @pytest.fixture(scope="module")
 def emul():
-    os.makedirs(BUILD, exist_ok=True)
-    hdr = os.path.join(BUILD, "hmpc_device_host.cuh")
-    with open(hdr, "w") as f:
-        f.write(_host_buildable(open(DEVICE_HEADER).read()))
-    lib = os.path.join(BUILD, "libkernel_source_on_host.so")
-    cmd = ["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-w", "-pthread",
-           "-I" + os.path.join(HERE, "fake_cuda"), "-I" + os.path.join(ROOT, "include"),
-           '-DHMPC_DEVICE_HEADER="%s"' % hdr, os.path.join(HERE, "kernel_source_on_host.cpp"), "-o", lib,
-           "-l:libstdc++.so.6"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    L = ctypes.CDLL(lib)
-    L.emul_leg_torque.restype = ctypes.c_double
-    return L
+    return host_emulation()
 
 
 def _p(a):
-    return a.ctypes.data_as(ctypes.c_void_p)
+    return None if a is None else a.ctypes.data_as(ctypes.c_void_p)
+
+
+def emul_solve(L, N, packed=None, raw=None, hostlists=False, refine=False, mask=None, ws=None, warm=False, shift=1,
+               shifts=None, w=None, w64=None, st=None, tau=None, dump=None):
+    """One solve call of the library on the host (kernel_source_on_host.cpp, emul_solve): the device-resident chain over
+    packed records, or over the update_data_t records `raw` in place; hostlists=True: the host-buffer modes' launches over
+    host-built lists.  Outputs are written in place; w and st are allocated when not given.  -> (w, st, launched[4]:
+    instances class 0 kept, class 1, class 2, the refinement class)"""
+    B = len(packed if packed is not None else raw)
+    w = np.zeros((B, 12 * N), np.float32) if w is None else w
+    st = np.full(B, -1, np.int32) if st is None else st
+    launched = np.zeros(4, np.int32)
+    d = [dump[k] for k in ("H", "g", "Fblk", "lb", "ub")] if dump else [None] * 5
+    rc = L.emul_solve(_p(packed), _p(raw), B, N, int(hostlists), int(refine), _p(mask), _p(ws), int(warm), shift, _p(shifts),
+                      _p(w), _p(w64), _p(st), _p(tau), _p(launched), *[_p(a) for a in d])
+    assert rc == 0, rc
+    return w, st, launched
 
 
 def _prepare(L, states, N, dt_mpc=0.04):
@@ -246,16 +292,12 @@ def _solve(L, records, N, dump=False, tau=True):
     w = np.zeros((B, n), np.float32)
     st = np.full(B, -1, np.int32)
     t = np.zeros((B, 10), np.float32)
-    launched = np.zeros(3, np.int32)
     d = None
     if dump:
         d = dict(H=np.zeros((B, n, n), np.float32), g=np.zeros((B, n), np.float32), Fblk=np.zeros((B, 16, 12), np.float32),
                  lb=np.zeros((B, 16 * N), np.float32), ub=np.zeros((B, 16 * N), np.float32))
-    ptrs = [_p(d[k]) for k in ("H", "g", "Fblk", "lb", "ub")] if dump else [None] * 5
-    rc = L.emul_solve(_p(packed), B, N, ctypes.c_float(0.04), ctypes.c_float(500.0), 500, _p(w), _p(st), _p(t) if tau else None,
-                      _p(launched), *ptrs)
-    assert rc == 0
-    return w.astype(np.float64), st, t.astype(np.float64), launched, d
+    _, _, launched = emul_solve(L, N, packed, w=w, st=st, tau=t if tau else None, dump=d)
+    return w.astype(np.float64), st, t.astype(np.float64), launched[:3], d
 
 
 def _solve_plain(L, records, N):
@@ -383,14 +425,7 @@ def test_solve_kernel_source_has_no_data_races(emul, tmp_path):
     threads), the in-place gather mode with double stores, the warm start."""
     from conftest import load_golden
 
-    exe = os.path.join(BUILD, "race_driver_tsan")
-    cmd = ["g++", "-std=c++17", "-O1", "-g", "-ffp-contract=off", "-fsanitize=thread", "-w", "-pthread",
-           "-I" + os.path.join(HERE, "fake_cuda"), "-I" + os.path.join(ROOT, "include"),
-           '-DHMPC_DEVICE_HEADER="%s"' % os.path.join(BUILD, "hmpc_device_host.cuh"),
-           os.path.join(HERE, "kernel_source_on_host.cpp"), os.path.join(HERE, "race_driver.cpp"), "-o", exe]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        pytest.skip("no ThreadSanitizer runtime with this toolchain: " + r.stderr[-300:])
+    exe = race_driver()
     cases = [("cfg2_h10", [0, 1, 2], ()), ("cfg1_h10", [0], ()), ("degenerate_zero_force_h10", [0], ()),
              ("cfg4_h5", [0, 1, 2, 3], ()), ("cfg4_h16", [0, 1, 2], ()),       # runtime horizons: 64/224 and 224/544 threads
              ("cfg3_h10", [0, 1], ("raw",)),          # in-place gather of update_data_t records, double results
@@ -493,7 +528,8 @@ def test_solve_kernel_source_is_insensitive_to_its_two_tolerances(emul):
 
 def test_solve_kernel_source_in_place_and_warm_start_modes(emul):
     """The other modes of the same kernel: gathering the live bytes of the caller's update_data_t records in place (the
-    host-buffer path's in-place mode), double-precision result stores, and the optional S-pair warm start."""
+    device-resident chain of the host-buffer path's in-place mode), double-precision result stores, the launches over
+    host-built lists (the zero-copy and copy-pipeline modes) and the optional S-pair warm start."""
     from conftest import load_golden, rel_err
 
     g = load_golden("cfg3_h10")
@@ -504,18 +540,17 @@ def test_solve_kernel_source_in_place_and_warm_start_modes(emul):
     w64 = np.zeros((B, 12 * N), np.float64)
     st = np.full(B, -1, np.int32)
     tau = np.zeros((B, 10), np.float32)
-    rc = emul.emul_solve_ex(None, _p(recs), B, N, ctypes.c_float(0.04), ctypes.c_float(500.0), 500, 0, _p(w), _p(w64), _p(st), _p(tau),
-                            None, None, None, None, None, None)
-    assert rc == 0
+    emul_solve(emul, N, raw=recs, w=w, w64=w64, st=st, tau=tau)
     assert np.array_equal(w.astype(np.float64), w0) and np.array_equal(st, st0) and np.array_equal(tau.astype(np.float64), tau0)
     assert np.array_equal(w64.astype(np.float32), w)   # the double store keeps the fp64 solve's bits; rounded it is the float result
     assert np.abs(w64 - w0).max() > 0                  # ... and it is not just the float result widened
     packed = np.ascontiguousarray(interface.pack_records(recs, N))
+    wh, sh, launched = emul_solve(emul, N, packed, hostlists=True)
+    assert np.array_equal(wh.astype(np.float64), w0) and np.array_equal(sh, st0) and launched[:2].sum() == B
     ww = np.zeros((B, 12 * N), np.float32)
     sw = np.full(B, -1, np.int32)
-    rc = emul.emul_solve_ex(_p(packed), None, B, N, ctypes.c_float(0.04), ctypes.c_float(500.0), 500, 1, _p(ww), None, _p(sw), None,
-                            None, None, None, None, None, None)
-    assert rc == 0 and (interface.status_code(sw) == 0).all()
+    emul_solve(emul, N, packed, warm=True, w=ww, st=sw)   # (no working-set memory: the warm flag proposes nothing)
+    assert (interface.status_code(sw) == 0).all()
     assert rel_err(ww.astype(np.float64), g["q_soln"][:B]).max() < 5e-5
 
 
@@ -538,8 +573,7 @@ def test_closed_loop_of_kernel_sources(emul, oracle):
     def solve(packed):
         w = np.zeros((B, 12 * N), np.float32)
         st = np.full(B, -1, np.int32)
-        assert emul.emul_solve(_p(packed), B, N, ctypes.c_float(0.04), ctypes.c_float(500.0), 500, _p(w), _p(st), None, None,
-                               None, None, None, None, None) == 0
+        emul_solve(emul, N, packed, w=w, st=st)
         assert (interface.status_code(st) == 0).all()
         return w, st
 
@@ -563,12 +597,7 @@ def test_closed_loop_of_kernel_sources(emul, oracle):
         # warm loop
         packed = np.zeros((B, stride), np.uint8)
         emul.emul_prepare(_p(s_w), B, N, ctypes.c_double(0.04), _p(packed))
-        emul.emul_set_ws(_p(ws), 1)
-        w_w = np.zeros((B, 12 * N), np.float32)
-        st_w = np.full(B, -1, np.int32)
-        assert emul.emul_solve_ex(_p(packed), None, B, N, ctypes.c_float(0.04), ctypes.c_float(500.0), 500, 1, _p(w_w), None, _p(st_w),
-                                  None, None, None, None, None, None, None) == 0
-        emul.emul_set_ws(None, 0)
+        w_w, st_w, _ = emul_solve(emul, N, packed, ws=ws, warm=True, shift=1)
         assert (interface.status_code(st_w) == 0).all()
         assert np.abs(w_w.astype(np.float64) - w_k).max() < 1e-5 * np.abs(w_k).max()   # same optimum (float output)
         if t > 0:
@@ -601,15 +630,7 @@ def test_solve_kernel_source_warm_start_survives_any_proposal(emul):
     W = emul.emul_ws_ints()
 
     def run(ws, shift):
-        w = np.zeros((B, 12 * N), np.float32)
-        st = np.full(B, -1, np.int32)
-        emul.emul_set_ws(_p(ws) if ws is not None else None, shift)
-        try:
-            rc = emul.emul_solve_ex(_p(packed), None, B, N, ctypes.c_float(0.04), ctypes.c_float(500.0), 500, 1 if ws is not None else 0,
-                                    _p(w), None, _p(st), None, None, None, None, None, None, None)
-        finally:
-            emul.emul_set_ws(None, 0)
-        assert rc == 0
+        w, st, _ = emul_solve(emul, N, packed, ws=ws, warm=ws is not None, shift=shift)
         return w.astype(np.float64), st
 
     w0, st0 = run(None, 0)
@@ -699,3 +720,55 @@ def test_solve_kernel_source_reports_a_hessian_beyond_its_conditioning_limit(emu
     finally:
         del os.environ["HMPC_KAPPA_MAX"]
     assert interface.status_code(st).tolist() == [0] and 1e-3 < rel_err(w, ref, 12)[0] < 5e-2
+
+
+# ---- the class shapes of the shared planner (hmpc_chain.h plan_classes) ---------------------------------------------------
+# horizon: (size classes, [(variant, threads, dynamic smem bytes, working-set capacity, blocks of 6 variables, cached
+# columns) of classes 0 ..], the same of the refinement class) — the shapes the library has launched since the refinement
+# class came in.
+CLASS_SHAPES = {
+    1: (2, [(10, 64, 6336, 6, 1, 5), (15, 64, 7472, 12, 2, 12)], (20, 64, 8336, 12, 2, 0)),
+    2: (2, [(10, 64, 7888, 8, 2, 6), (15, 64, 13408, 24, 4, 24)], (20, 64, 11904, 24, 4, 0)),
+    3: (3, [(10, 64, 10144, 10, 3, 7), (16, 128, 24544, 31, 6, 31), (16, 128, 19136, 36, 6, 0)], (21, 128, 23264, 36, 6, 0)),
+    4: (3, [(10, 64, 10416, 12, 4, 8), (16, 128, 30880, 31, 8, 31), (16, 128, 25184, 48, 8, 0)], (21, 128, 30944, 48, 8, 0)),
+    5: (3, [(10, 64, 13408, 14, 5, 9), (16, 128, 41888, 31, 10, 31), (16, 128, 38976, 60, 10, 0)], (21, 128, 48672, 60, 10, 0)),
+    6: (3, [(11, 128, 19168, 16, 6, 10), (17, 192, 49760, 31, 12, 31), (17, 192, 50784, 72, 12, 0)], (22, 192, 62880, 72, 12, 0)),
+    7: (3, [(11, 128, 19728, 18, 7, 11), (17, 192, 63840, 31, 14, 31), (17, 192, 69952, 84, 14, 0)], (22, 192, 87520, 84, 14, 0)),
+    8: (3, [(11, 128, 20864, 20, 8, 12), (17, 192, 73248, 31, 16, 31), (17, 192, 85600, 96, 16, 0)], (22, 192, 106336, 96, 16, 0)),
+    9: (3, [(11, 128, 26064, 22, 9, 13), (18, 256, 90400, 31, 18, 31), (18, 256, 110144, 108, 18, 0)], (23, 256, 137888, 108, 18, 0)),
+    10: (3, [(0, 128, 31920, 24, 10, 14), (1, 256, 101344, 31, 20, 31), (18, 256, 129632, 120, 20, 0)], (23, 256, 161312, 120, 20, 0)),
+    11: (3, [(12, 192, 38400, 26, 11, 15), (19, 384, 124992, 96, 22, 0), (19, 384, 159552, 132, 22, 0)], (24, 384, 199776, 132, 22, 0)),
+    12: (3, [(12, 192, 40336, 28, 12, 16), (19, 384, 134496, 96, 24, 0), (19, 384, 182880, 144, 24, 0)], (24, 384, 227808, 144, 24, 0)),
+    13: (3, [(12, 192, 47584, 30, 13, 17), (19, 384, 154816, 96, 26, 0), (19, 384, 218176, 156, 26, 0)], (24, 384, 227744, 116, 26, 0)),
+    14: (3, [(12, 192, 55488, 32, 14, 18), (19, 384, 165856, 96, 28, 0), (19, 384, 229216, 156, 28, 0)], (24, 384, 229664, 100, 28, 0)),
+    15: (3, [(12, 192, 64016, 34, 15, 19), (19, 384, 189248, 96, 30, 0), (19, 384, 228288, 136, 30, 0)], (22, 192, 101488, 90, 15, 0)),
+    16: (3, [(12, 192, 66464, 36, 16, 20), (19, 384, 201824, 96, 32, 0), (19, 384, 227808, 124, 32, 0)], (22, 192, 106400, 96, 16, 0)),
+}
+
+
+@pytest.mark.parametrize("horizon", sorted(CLASS_SHAPES))
+def test_class_planner_keeps_the_shapes(emul, horizon):
+    """Every horizon the library accepts: the number of size classes and every class's kernel variant, threads, shared
+    memory, working-set capacity, blocks and cached columns, refinement class included."""
+    out = np.zeros((4, 6), np.int32)
+    ncls = emul.emul_plan(horizon, _p(out))
+    want_ncls, want, want_ref = CLASS_SHAPES[horizon]
+    assert ncls == want_ncls
+    assert [tuple(r) for r in out[:ncls].tolist()] == want
+    assert tuple(out[3].tolist()) == want_ref
+
+
+@pytest.mark.gpu
+def test_class_config_on_the_device_is_the_planners():
+    """hmpc_class_config of a context of every horizon: the planner's threads, shared memory, working-set capacity and
+    blocks, and room for at least one resident CTA."""
+    for horizon, (ncls, want, want_ref) in sorted(CLASS_SHAPES.items()):
+        mpc = interface.BatchedMPC(4, horizon)
+        try:
+            assert mpc.launches_per_solve == ncls
+            for cls, row in [(i, want[i]) for i in range(ncls)] + [(interface.REFINEMENT_CLASS, want_ref)]:
+                cfg = mpc.class_config(cls)
+                assert (cfg["threads"], cfg["smem_bytes"], cfg["qmax"], cfg["nb_cap"]) == row[1:5], (horizon, cls, cfg)
+                assert cfg["grid_cap"] > 0, (horizon, cls, cfg)
+        finally:
+            mpc.close()

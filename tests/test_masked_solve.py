@@ -1,7 +1,7 @@
 """Solving part of the batch: hmpc_solve_device_masked, hmpc_solve_batch_masked, BatchedMPC.solve_device_masked and
 BatchedMPC.solve_batch_masked solve robot i iff mask[i] != 0 and leave every other robot's results and working set alone.
 
-CPU: the kernel source (tests/host_emul/masked_on_host.cpp) — the selection kernel gives np.flatnonzero(mask) on one
+CPU: the kernel source (tests/host_emul/kernel_source_on_host.cpp) — the selection kernel gives np.flatnonzero(mask) on one
 emulated CTA (also under ThreadSanitizer), and a masked solve of walking and double-support robots gives the listed robots
 a full solve's results, status words and working sets while the unlisted keep sentinel bytes.  GPU: the library — a full
 mask against hmpc_solve_device_warm, random masks on a batch that reaches classes 1 and 2, a staggered warm loop against
@@ -14,9 +14,9 @@ import subprocess
 import numpy as np
 import pytest
 
-from conftest import GOLDEN, ROOT, load_golden
+from conftest import GOLDEN, load_golden
 from hector_simulation_b200 import interface, scenarios
-from test_kernel_source_on_host import BUILD, DEVICE_HEADER, HERE, _host_buildable, _p
+from test_kernel_source_on_host import _p, emul_solve, host_emulation, race_driver
 
 N = 10
 W_SENT, S_SENT, WS_SENT = np.uint32(0x7FA5A5A5), np.int32(0x5A5A5A5A), np.int32(0x3C3C3C3C)
@@ -30,18 +30,7 @@ def _bits(a):
 # ---- CPU: the kernel source on the host ----------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emul():
-    """tests/host_emul/masked_on_host.cpp, built for the host the way test_kernel_source_on_host.py builds its driver."""
-    os.makedirs(BUILD, exist_ok=True)
-    hdr = os.path.join(BUILD, "hmpc_device_host_masked.cuh")
-    with open(hdr, "w") as f:
-        f.write(_host_buildable(open(DEVICE_HEADER).read()))
-    lib = os.path.join(BUILD, "libmasked_on_host.so")
-    cmd = ["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-w", "-pthread",
-           "-I" + os.path.join(HERE, "fake_cuda"), "-I" + os.path.join(ROOT, "include"),
-           '-DHMPC_DEVICE_HEADER="%s"' % hdr, os.path.join(HERE, "masked_on_host.cpp"), "-o", lib, "-l:libstdc++.so.6"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return ctypes.CDLL(lib)
+    return host_emulation()
 
 
 def _select(L, mask):
@@ -78,36 +67,21 @@ def test_select_source_gives_the_listed_robots_in_order(emul, name, mask):
 def test_select_source_has_no_data_races(emul, tmp_path):
     """ThreadSanitizer build of the selection kernel (every CUDA thread an OS thread, every barrier real) on masks of 1 to
     1300 robots and four densities."""
-    exe = os.path.join(BUILD, "masked_race_driver_tsan")
-    cmd = ["g++", "-std=c++17", "-O1", "-g", "-ffp-contract=off", "-fsanitize=thread", "-w", "-pthread", "-DMASKED_RACE_MAIN",
-           "-I" + os.path.join(HERE, "fake_cuda"), "-I" + os.path.join(ROOT, "include"),
-           '-DHMPC_DEVICE_HEADER="%s"' % os.path.join(BUILD, "hmpc_device_host_masked.cuh"),
-           os.path.join(HERE, "masked_on_host.cpp"), "-o", exe]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        pytest.skip("no ThreadSanitizer runtime with this toolchain: " + r.stderr[-300:])
+    exe = race_driver()
     env = dict(os.environ, TSAN_OPTIONS="halt_on_error=0 exitcode=66")
-    r = subprocess.run([exe], capture_output=True, text=True, env=env, timeout=1800)
+    r = subprocess.run([exe, "select"], capture_output=True, text=True, env=env, timeout=1800)
     assert "ThreadSanitizer" not in r.stderr, r.stderr[:3000]
     assert r.returncode == 0 and r.stdout.strip() == "ok", (r.returncode, r.stdout)
 
 
 def _emul_full(L, packed, ws, shifts):
-    B = len(packed)
-    w = np.zeros((B, 12 * N), np.float32)
-    st = np.zeros(B, np.int32)
-    la = np.zeros(3, np.int32)
-    assert L.emul_solve_warm(_p(packed), B, N, ctypes.c_float(0.04), ctypes.c_float(500.0), 500, _p(ws), 1, _p(shifts),
-                             _p(w), _p(st), _p(la)) == 0
-    return w, st, la
+    w, st, la = emul_solve(L, N, packed, ws=ws, warm=True, shifts=shifts)
+    return w, st, la[:3]
 
 
 def _emul_masked(L, packed, mask, ws, shifts, w, st):
-    la = np.zeros(3, np.int32)
-    rc = L.emul_solve_masked(_p(packed), len(packed), N, _p(np.ascontiguousarray(mask, np.uint8)), _p(ws), _p(shifts),
-                             _p(w), _p(st), _p(la))
-    assert rc == 0
-    return la
+    _, _, la = emul_solve(L, N, packed, mask=np.ascontiguousarray(mask, np.uint8), ws=ws, warm=True, shifts=shifts, w=w, st=st)
+    return la[:3]
 
 
 def test_masked_source_solves_the_listed_robots_only(emul):

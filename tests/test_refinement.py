@@ -1,7 +1,7 @@
 """Robots beyond the conditioning limit of the sweep inversion: the opt-in refinement class (hmpc_set_refinement,
 hmpc_reference_set_refinement, BatchedMPC.set_refinement, interface.reference_set_refinement).
 
-CPU: the kernel source (tests/host_emul/refine_on_host.cpp: the device-resident chain with the refinement class at its end)
+CPU: the kernel source (tests/host_emul/kernel_source_on_host.cpp: the device-resident chain with the refinement class at its end)
 against the fp64 referee — the lying robot of stress_referee.npz, a generated batch of fallen and tilted robots spanning
 scaled condition numbers of up to 1.6e6 (single and double support, horizons 8 and 10), well-conditioned robots untouched
 bit for bit, a non-positive pivot not handed over, and a ThreadSanitizer run.  GPU: the same through the library — the
@@ -13,9 +13,9 @@ import subprocess
 import numpy as np
 import pytest
 
-from conftest import GOLDEN, ROOT, load_golden, rel_err
+from conftest import GOLDEN, load_golden, rel_err
 from hector_simulation_b200 import interface, scenarios
-from test_kernel_source_on_host import BUILD, DEVICE_HEADER, HERE, _host_buildable, _p
+from test_kernel_source_on_host import _p, emul_solve, host_emulation, race_driver
 
 N = 10
 KAPPA_REFINE, KAPPA_MAX, KAPPA_MAX_REFINED = 1.5e4, 1.5e5, 1e9   # hmpc_capi.cu's defaults
@@ -65,33 +65,16 @@ def _referee(recs, horizon):
 # ---- CPU: the kernel source on the host ----------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emul():
-    """tests/host_emul/refine_on_host.cpp, built for the host the way test_kernel_source_on_host.py builds its driver."""
-    os.makedirs(BUILD, exist_ok=True)
-    hdr = os.path.join(BUILD, "hmpc_device_host_refine.cuh")
-    with open(hdr, "w") as f:
-        f.write(_host_buildable(open(DEVICE_HEADER).read()))
-    lib = os.path.join(BUILD, "librefine_on_host.so")
-    cmd = ["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-w", "-pthread",
-           "-I" + os.path.join(HERE, "fake_cuda"), "-I" + os.path.join(ROOT, "include"),
-           '-DHMPC_DEVICE_HEADER="%s"' % hdr, os.path.join(HERE, "refine_on_host.cpp"), "-o", lib, "-l:libstdc++.so.6"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return ctypes.CDLL(lib)
+    return host_emulation()
 
 
 def _emul_solve(L, recs, horizon, refine, ws=None, warm=0):
     """the device-resident chain on the host -> (wrench f64 [B,12N] (the kernel's double stores), status, ws, launched[4])"""
     B = len(recs)
     packed = np.ascontiguousarray(interface.pack_records(recs, horizon))
-    w = np.zeros((B, 12 * horizon), np.float32)
     w64 = np.zeros((B, 12 * horizon))
-    st = np.full(B, -1, np.int32)
-    la = np.zeros(4, np.int32)
     ws = np.zeros((B, L.emul_ws_ints()), np.int32) if ws is None else ws
-    rc = L.emul_solve_refine(_p(packed), B, horizon, ctypes.c_float(0.04), ctypes.c_float(500.0), 1 if refine else 0,
-                             ctypes.c_double(KAPPA_MAX), ctypes.c_double(KAPPA_REFINE), ctypes.c_double(KAPPA_MAX_REFINED),
-                             _p(ws), warm, _p(w), _p(w64), _p(st), _p(la))
-    assert rc == 0
+    w, st, la = emul_solve(L, horizon, packed, refine=refine, ws=ws, warm=warm, w64=w64)   # the library's default kappas
     assert np.array_equal(w64.astype(np.float32).view(np.uint32), w.view(np.uint32))
     return w64, st, ws, la
 
@@ -183,19 +166,12 @@ def test_refinement_source_rollout_start_of_lying_robots(emul):
 def test_refinement_source_has_no_data_races(emul, tmp_path):
     """ThreadSanitizer build of the driver (every CUDA thread an OS thread, every barrier real) on h10_lying with
     refinement on: class 0 hands it over, the refinement class solves it."""
-    exe = os.path.join(BUILD, "refine_race_driver_tsan")
-    cmd = ["g++", "-std=c++17", "-O1", "-g", "-ffp-contract=off", "-fsanitize=thread", "-w", "-pthread", "-DREFINE_RACE_MAIN",
-           "-I" + os.path.join(HERE, "fake_cuda"), "-I" + os.path.join(ROOT, "include"),
-           '-DHMPC_DEVICE_HEADER="%s"' % os.path.join(BUILD, "hmpc_device_host_refine.cuh"),
-           os.path.join(HERE, "refine_on_host.cpp"), "-o", exe]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        pytest.skip("no ThreadSanitizer runtime with this toolchain: " + r.stderr[-300:])
+    exe = race_driver()
     recs, _ = _lying()
     f = tmp_path / "lying.bin"
     np.ascontiguousarray(interface.pack_records(recs, N)).tofile(f)
     env = dict(os.environ, TSAN_OPTIONS="halt_on_error=0 exitcode=66")
-    r = subprocess.run([exe, str(f), str(N)], capture_output=True, text=True, env=env, timeout=1800)
+    r = subprocess.run([exe, str(f), str(N), "refine"], capture_output=True, text=True, env=env, timeout=1800)
     assert "ThreadSanitizer" not in r.stderr, r.stderr[:3000]
     assert r.returncode == 0 and "launched 1 0 0 1" in r.stdout, (r.returncode, r.stdout)
     st = int(r.stdout.split("status")[1].split()[0], 16)

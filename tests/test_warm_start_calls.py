@@ -1,50 +1,28 @@
 """Warm start in the caller's own loop: hmpc_solve_device_warm, hmpc_solve_batch_warm and the reference boundary after
 hmpc_reference_set_warm_start(1).
 
-CPU: the kernel source (tests/host_emul/warm_start_on_host.cpp) with per-robot shifts — a negative shift is a cold solve
+CPU: the kernel source (tests/host_emul/kernel_source_on_host.cpp) with per-robot shifts — a negative shift is a cold solve
 that still records its working set, mixed shifts in one batch equal per-robot runs, an instance that overflows class 0
 reaches class 1 with its proposal, and horizon 16 (no block start) is unaffected.  GPU: the calls against the device
 rollout they generalise, against cold solves of the same records, against each other (device / host-buffer modes /
 reference boundary), and with robots reset mid-loop."""
-import ctypes
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
 from conftest import GOLDEN, load_golden, rel_err
 from hector_simulation_b200 import interface, scenarios
-from test_kernel_source_on_host import BUILD, DEVICE_HEADER, HERE, _host_buildable, _p
+from test_kernel_source_on_host import emul_solve, host_emulation
 
 
 @pytest.fixture(scope="module")
 def emul():
-    """tests/host_emul/warm_start_on_host.cpp (the kernel-source driver plus the per-robot-shift solve), built for the host
-    the way test_kernel_source_on_host.py builds its driver."""
-    os.makedirs(BUILD, exist_ok=True)
-    hdr = os.path.join(BUILD, "hmpc_device_host_warm.cuh")
-    with open(hdr, "w") as f:
-        f.write(_host_buildable(open(DEVICE_HEADER).read()))
-    lib = os.path.join(BUILD, "libwarm_start_on_host.so")
-    cmd = ["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-w", "-pthread",
-           "-I" + os.path.join(HERE, "fake_cuda"), "-I" + os.path.join(os.path.dirname(os.path.dirname(HERE)), "include"),
-           '-DHMPC_DEVICE_HEADER="%s"' % hdr, os.path.join(HERE, "warm_start_on_host.cpp"), "-o", lib, "-l:libstdc++.so.6"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return ctypes.CDLL(lib)
+    return host_emulation()
 
 
 def _emul_solve(L, packed, N, ws=None, shift=0, shifts=None):
     """The device-resident path on the host; with `ws` the warm flag is on (scalar `shift`, or per-robot `shifts`)."""
-    B = len(packed)
-    w = np.zeros((B, 12 * N), np.float32)
-    st = np.full(B, -1, np.int32)
-    launched = np.zeros(3, np.int32)
-    rc = L.emul_solve_warm(_p(packed), B, N, ctypes.c_float(0.04), ctypes.c_float(500.0), 500, _p(ws) if ws is not None else None,
-                           shift, _p(shifts) if shifts is not None else None, _p(w), _p(st), _p(launched))
-    assert rc == 0
-    return w, st, launched
+    w, st, launched = emul_solve(L, N, packed, ws=ws, warm=ws is not None, shift=shift, shifts=shifts)
+    return w, st, launched[:3]
 
 
 def _sets(ws):
