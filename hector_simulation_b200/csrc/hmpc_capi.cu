@@ -256,6 +256,15 @@ int launch_class(const hmpc_ctx* c, int cls, const hmpc::SolveIO& io, const hmpc
   return HMPC_OK;
 }
 
+// the preparation kernel (hmpc_chain.h: prepare_args) on one thread per robot or list entry at most
+int launch_prepare(const hmpc::PrepareArgs& pa, cudaStream_t st, bool pdl)
+{
+  CK(launch_chain(hmpc::hmpc_prepare_kernel, dim3(hmpc::prepare_grid(pa.batch)), dim3(hmpc::PREPARE_THREADS), 0, st, pdl,
+                  pa.states, pa.batch, pa.N, pa.dtMPC, pa.records, pa.rec_stride, pa.list, pa.count));
+  CK(cudaGetLastError());
+  return HMPC_OK;
+}
+
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------
@@ -555,7 +564,7 @@ namespace {
 constexpr int CAPTURE_SLOT = 1;
 static_assert(CAPTURE_SLOT < NCHUNK, "d_cls holds NCHUNK slots");
 // The device-resident chain: one launch per class, all enqueued on `st`; with io.mask (device-readable [B]) the selection
-// kernel first.  No classification kernel: the class-0 launch runs over every instance (or, in a masked call, over the list
+// kernel first, and with io.states the preparation of the robots class 0 runs over (hmpc_chain.h).  No classification kernel: the class-0 launch runs over every instance (or, in a masked call, over the list
 // the selection kernel built from the mask) and hands the ones with more stance blocks than it holds to class 1's list.
 // An eager chain uses the parity of its call count: the previous call's class-0 launch zeroed those lengths.  A graph
 // replays the lengths it was recorded with and nothing zeroes them between replays, so a chain recorded into a graph
@@ -580,6 +589,10 @@ int enqueue_solve(hmpc_ctx* c, const hmpc::SolveIO& io, cudaStream_t st)
     CK(launch_chain(hmpc::hmpc_select_kernel<hmpc::SELECT_THREADS>, dim3(1), dim3(hmpc::SELECT_THREADS), 0, st, pdl, io.mask,
                     io.batch, s.list0(), s.counts()));
     CK(cudaGetLastError());
+  }
+  if (io.states) {
+    // the states chain: records of the listed robots (every robot without a mask) into io.records, read by class 0
+    if (int rc = launch_prepare(hmpc::prepare_args(c->horizon, io, lists), st, pdl)) return rc;
   }
   for (int i = 0; i < c->ncls; i++)
     if (int rc = launch_class(c, i, io, lists, io.batch, st, pdl)) return rc;
@@ -813,11 +826,30 @@ HMPC_EXTERNC int hmpc_prepare_device(hmpc_ctx* c, const hmpc_state_t* d_states, 
   if (!c || !d_states || !d_records || B < 0) { g_err = "hmpc_prepare_device: bad argument"; return HMPC_ERR_ARG; }
   if (B == 0) return HMPC_OK;
   CK(cudaSetDevice(c->device));
-  hmpc::hmpc_prepare_kernel<<<(B + 63) / 64, 64, 0, static_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const unsigned char*>(d_states), B, c->horizon, dtMPC,
-      static_cast<unsigned char*>(d_records), c->rec_stride);
-  CK(cudaGetLastError());
-  return HMPC_OK;
+  hmpc::SolveIO io;
+  io.states = d_states;
+  io.records = d_records;
+  io.batch = B;
+  io.dt_mpc = dtMPC;
+  return launch_prepare(hmpc::prepare_args(c->horizon, io, hmpc::ChainLists{}), static_cast<cudaStream_t>(stream), false);
+}
+
+HMPC_EXTERNC int hmpc_solve_states_device_masked(hmpc_ctx* c, const hmpc_state_t* d_states, int B, const unsigned char* d_mask,
+                                                 double dtMPC, void* d_records, float* d_wrench, int* d_status, float* d_tau,
+                                                 const int* d_shift, void* stream)
+{
+  if (!c || !d_states || !d_mask || !d_records || !d_wrench || !d_status || B < 0) {
+    g_err = "hmpc_solve_states_device_masked: bad argument";
+    return HMPC_ERR_ARG;
+  }
+  if (B == 0) return HMPC_OK;
+  if (int rc = check_device_records(c, d_records, B, "hmpc_solve_states_device_masked")) return rc;
+  hmpc::SolveIO io = device_call(c, d_records, B, d_wrench, d_status, d_tau, true);
+  io.shifts = d_shift;
+  io.mask = d_mask;
+  io.states = d_states;
+  io.dt_mpc = dtMPC;
+  return enqueue_solve(c, io, static_cast<cudaStream_t>(stream));
 }
 
 HMPC_EXTERNC int hmpc_pin_host_buffer(hmpc_ctx* c, void* ptr, size_t bytes)
@@ -945,6 +977,20 @@ HMPC_EXTERNC int hmpc_solve_batch_states(hmpc_ctx* c, const hmpc_state_t* in, in
   return solve_batch_impl(c, nullptr, in, B, wrench_out, tau_out, status, dtMPC);
 }
 
+HMPC_EXTERNC int hmpc_solve_batch_states_warm(hmpc_ctx* c, const hmpc_state_t* in, int B, double dtMPC, double* wrench_out,
+                                              double* tau_out, int* status, const int* shift)
+{
+  if (!in) { g_err = "hmpc_solve_batch_states_warm: bad argument (null states)"; return HMPC_ERR_ARG; }
+  return solve_batch_impl(c, nullptr, in, B, wrench_out, tau_out, status, dtMPC, true, shift);
+}
+
+HMPC_EXTERNC int hmpc_solve_batch_states_masked(hmpc_ctx* c, const hmpc_state_t* in, int B, const unsigned char* mask,
+                                                double dtMPC, double* wrench_out, double* tau_out, int* status, const int* shift)
+{
+  if (!in || !mask) { g_err = "hmpc_solve_batch_states_masked: bad argument (null states or mask)"; return HMPC_ERR_ARG; }
+  return solve_batch_impl(c, nullptr, in, B, wrench_out, tau_out, status, dtMPC, true, shift, mask);
+}
+
 // mask (hmpc_solve_batch_masked) or NULL: only the robots it lists are solved, and only their rows of wrench_out, tau_out and
 // status are written; the context's staging rows of the others keep stale results, which nothing reads
 static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_state_t* sin, int B, double* wrench_out,
@@ -988,17 +1034,21 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
     memcpy(c->h_shift, shift, (size_t)B * sizeof(int));
     hsh = c->h_shift;
   }
-  // in-place mode: records, wrenches and status all live in buffers the caller registered (hmpc_pin_host_buffer):
-  // the kernels gather the live bytes of every update_data_t over PCIe and store double results where the caller
-  // wants them — the call is host classification + launches + one synchronize
-  if (in && zc_env != 0 && !c->pins.empty() && c->pinned(in, (size_t)B * sizeof(update_data_t)) &&
-      c->pinned(wrench_out, (size_t)B * nw * sizeof(double)) && (!status || c->pinned(status, (size_t)B * sizeof(int)))) {
-    // the device-resident chain on the caller's records: class 0 classifies on the way, overflow escalates on the device
+  // in-place mode: records (or states), wrenches and status all live in buffers the caller registered
+  // (hmpc_pin_host_buffer): the kernels gather the live bytes of every update_data_t over PCIe, or the preparation kernel
+  // reads the states there, and double results are stored where the caller wants them — the call is launches + one
+  // synchronize
+  const bool in_pinned = in ? c->pinned(in, (size_t)B * sizeof(update_data_t)) : c->pinned(sin, (size_t)B * sizeof(hmpc_state_t));
+  if (zc_env != 0 && !c->pins.empty() && in_pinned && c->pinned(wrench_out, (size_t)B * nw * sizeof(double)) &&
+      (!status || c->pinned(status, (size_t)B * sizeof(int)))) {
+    // the device-resident chain on the caller's records (states: prepared into the context's d_rec first): class 0
+    // classifies on the way, overflow escalates on the device
     int* ds = status ? status : reinterpret_cast<int*>(c->h_out + (size_t)c->max_batch * nw * 4);
     float* dt_ = tau_out ? reinterpret_cast<float*>(c->h_out + (size_t)c->max_batch * (nw * 4 + 4)) : nullptr;
     if (mask) memcpy(c->h_mask, mask, (size_t)B);  // pinned: the selection kernel reads it mapped
     hmpc::SolveIO io;
     io.raw = in;
+    if (sin) io.states = sin, io.records = c->d_rec, io.dt_mpc = dtMPC;
     io.batch = B;
     io.wrench = c->shard_out;
     io.wrench64 = wrench_out;
@@ -1039,7 +1089,8 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
     if (nb == 0) continue;
     int rc = HMPC_OK;
     if (sin) {
-      // row f-1: ship the 352-byte states and build the packed records on the device
+      // row f-1: ship the 352-byte states and build the packed records on the device (in a masked call the unlisted
+      // robots' records are built too, and not read)
       const size_t sb = sizeof(hmpc_state_t);
       memcpy(c->h_states + (size_t)b0 * sb, sin + b0, (size_t)nb * sb);
       if (trace) tr[ntr++] = now();
@@ -1085,7 +1136,9 @@ static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_sta
       io[k].shifts = c->d_shift + b0;
     }
     hblk[k] = c->h_cls + (size_t)k * hmpc::host_lists_ints(c->max_batch);
-    if (sin) hmpc::classify_host(c->horizon, c->cfg.f_max, c->cls[0].nb_hi, sin[b0].gait, sizeof(hmpc_state_t), nb, hblk[k], c->max_batch);
+    if (sin)
+      hmpc::classify_host(c->horizon, c->cfg.f_max, c->cls[0].nb_hi, sin[b0].gait, sizeof(hmpc_state_t), nb, hblk[k], c->max_batch,
+                          mask ? mask + b0 : nullptr);
     else
       hmpc::classify_host(c->horizon, c->cfg.f_max, c->cls[0].nb_hi, in[b0].gait, sizeof(update_data_t), nb, hblk[k], c->max_batch,
                           mask ? mask + b0 : nullptr);

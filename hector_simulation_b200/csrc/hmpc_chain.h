@@ -2,8 +2,11 @@
 // kernel source (tests/host_emul/kernel_source_on_host.cpp): the kernel variants, the shapes of the size classes, the
 // class-list memory and the arguments of every launch.  Host C++ only, no CUDA runtime calls; include hmpc_device.cuh first.
 //
-// One solve is a fixed sequence of launches: [selection kernel (masked calls)] -> class 0 (classifies on the way) ->
-// class 1 -> class 2 (reached by escalation) -> [refinement class (hmpc_set_refinement)].
+// One solve is a fixed sequence of launches: [selection kernel (masked calls)] -> [preparation (states in)] -> class 0
+// (classifies on the way) -> class 1 -> class 2 (reached by escalation) -> [refinement class (hmpc_set_refinement)].
+// A call with robot states (hmpc_state_t) in runs the preparation kernel over the selection kernel's class-0 list (or over
+// every robot) into the record buffer that class 0 then reads; preparation waits for the selection kernel, class 0 for
+// preparation.
 #pragma once
 #include <cstddef>
 
@@ -173,8 +176,10 @@ struct SolverSettings {
 
 // What one solve call hands its launches.  Unused pointers stay null.
 struct SolveIO {
-  const void* records = nullptr;             // packed records
+  const void* records = nullptr;             // packed records (with `states`: the buffer the preparation writes)
   const void* raw = nullptr;                 // or the caller's update_data_t records, read in place (3016-byte stride)
+  const void* states = nullptr;              // or hmpc_state_t [batch] (352-byte stride): the chain prepares `records`
+  double dt_mpc = 0.0;                       // the preparation's MPC step
   int batch = 0;
   float* wrench = nullptr;                   // [batch][12N] float results
   double* wrench64 = nullptr;                // [batch][12N] double results
@@ -225,6 +230,34 @@ inline ChainLists host_lists(int* block, int max_batch, int* ref, bool escalate)
   if (ref) l.ref_count = ref, l.ref_list = ref + 1;
   l.escalate = escalate;
   return l;
+}
+
+// The preparation launch of a states chain: every robot, or class 0's list when the selection kernel built one.  One
+// thread per list entry at most: launch prepare_grid(io.batch) CTAs of PREPARE_THREADS.
+constexpr int PREPARE_THREADS = 64;
+inline int prepare_grid(int batch) { return (batch + PREPARE_THREADS - 1) / PREPARE_THREADS; }
+// hmpc_prepare_kernel's parameters, in its order
+struct PrepareArgs {
+  const unsigned char* states;
+  int batch, N;
+  double dtMPC;
+  unsigned char* records;
+  int rec_stride;
+  const int* list;
+  const int* count;
+};
+inline PrepareArgs prepare_args(int N, const SolveIO& io, const ChainLists& lists)
+{
+  PrepareArgs pa{};
+  pa.states = static_cast<const unsigned char*>(io.states);
+  pa.batch = io.batch;
+  pa.N = N;
+  pa.dtMPC = io.dt_mpc;
+  pa.records = static_cast<unsigned char*>(const_cast<void*>(io.records));  // (written here, read by the classes)
+  pa.rec_stride = record_stride(N);
+  pa.list = lists.list[0];
+  pa.count = lists.list[0] ? lists.counts : nullptr;  // class 0's length word is counts[0]
+  return pa;
 }
 
 // The arguments of the launch of class `cls` (0-2, or REFINE_CLASS: the refinement class over lists.ref_list), shaped `k`.

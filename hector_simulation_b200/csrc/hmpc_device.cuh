@@ -620,13 +620,21 @@ __device__ __forceinline__ int tri(int s) { return s * (s + 1) / 2; }
 // row f-1: the caller's data preparation, one thread per robot (ConvexMPCLocomotion.cpp:283-406 followed by the
 // double -> float narrowing of update_problem_data, convexMPC_interface.cpp:87-99).  Double arithmetic with
 // explicitly rounded operations in the reference's order, so the packed record equals the host-prepared one.
-// `st` points at hmpc_state_t records (352 bytes): 39 doubles then the gait bytes.
+// `states` points at hmpc_state_t records (352 bytes): 39 doubles then the gait bytes.
 // ------------------------------------------------------------------------------------------------
+// Row i of `records` is robot i's record.  `list` and its length word `count` (the masked chain: the selection kernel's
+// class-0 list), or null: every robot in [0, batch).  With a list, thread t prepares robot list[t] for t < *count and no
+// other record is written.
 __global__ void hmpc_prepare_kernel(const unsigned char* states, int batch, int N, double dtMPC, unsigned char* records,
-                                    int rec_stride)
+                                    int rec_stride, const int* list = nullptr, const int* count = nullptr)
 {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= batch) return;
+  pdl_trigger();  // class 0 may become resident; it waits for this kernel before it reads the records
+  // In the chain, the list comes from the selection kernel, and the previous call's kernels may still read the record
+  // buffer: nothing is read or stored before they have completed.  A no-op for an ordinary launch.
+  pdl_wait();
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (list ? *count : batch)) return;
+  const int i = list ? list[t] : t;
   const double* s = reinterpret_cast<const double*>(states + (size_t)i * 352);
   const unsigned char* gait = states + (size_t)i * 352 + 39 * 8;
   const double* pos = s;            // [3]

@@ -32,6 +32,7 @@ EXPORTS = [
     "hmpc_solve_device_warm", "hmpc_solve_batch_warm", "hmpc_reference_set_warm_start",
     "hmpc_set_refinement", "hmpc_reference_set_refinement",
     "hmpc_solve_device_masked", "hmpc_solve_batch_masked",
+    "hmpc_solve_states_device_masked", "hmpc_solve_batch_states_warm", "hmpc_solve_batch_states_masked",
 ]
 REFINEMENT_CLASS = 3  # hmpc_class_config index of the refinement class (HMPC_REFINEMENT_CLASS)
 
@@ -124,6 +125,14 @@ def lib() -> ctypes.CDLL:
         L.hmpc_solve_device_masked.restype = ctypes.c_int
         L.hmpc_solve_batch_masked.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 5
         L.hmpc_solve_batch_masked.restype = ctypes.c_int
+        L.hmpc_solve_states_device_masked.argtypes = ([ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_double]
+                                                      + [ctypes.c_void_p] * 6)
+        L.hmpc_solve_states_device_masked.restype = ctypes.c_int
+        L.hmpc_solve_batch_states_warm.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_double] + [ctypes.c_void_p] * 4
+        L.hmpc_solve_batch_states_warm.restype = ctypes.c_int
+        L.hmpc_solve_batch_states_masked.argtypes = ([ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_double]
+                                                     + [ctypes.c_void_p] * 4)
+        L.hmpc_solve_batch_states_masked.restype = ctypes.c_int
         _lib = L
     return _lib
 
@@ -276,8 +285,8 @@ class BatchedMPC:
         return dict(zip(("threads", "smem_bytes", "qmax", "grid_cap", "nb_cap", "strip"), (int(v) for v in out)))
 
     def pin(self, *arrays: np.ndarray) -> None:
-        """Register caller-owned arrays (records, wrench, status) for the in-place mode of solve_batch: the GPU then
-        reads the records where they lie and writes the results where the caller wants them (hmpc_pin_host_buffer).
+        """Register caller-owned arrays (records or states, wrench, status) for the in-place mode of solve_batch and
+        solve_batch_states (and their _warm and _masked calls): the GPU then reads the records or states where they lie and writes the results where the caller wants them (hmpc_pin_host_buffer).
         The arrays must stay alive until unpin()/close().  Registration pins whole pages: allocate the arrays with
         page_aligned() so that no unrelated heap object shares their pages (a later cudaMemcpy of such a neighbour, partly
         inside a registered page range, fails with cudaErrorInvalidValue)."""
@@ -370,7 +379,8 @@ class BatchedMPC:
         return wrench, tau, status
 
     def solve_batch_states(self, states: np.ndarray, strict: bool = True, torques: bool = False, out=None, dt_mpc: float = 0.04):
-        """Row f-1: `hmpc_state_t` records in, data preparation on the device.  -> (wrench, [tau,] status)."""
+        """Row f-1: `hmpc_state_t` records in, data preparation on the device.  In place when the states, wrench and status
+        arrays are pinned (pin()).  -> (wrench, [tau,] status)."""
         from .scenarios import STATE_DTYPE
 
         if states.dtype != STATE_DTYPE or not states.flags.c_contiguous:
@@ -388,6 +398,50 @@ class BatchedMPC:
                                              tau.ctypes.data if torques else None, status.ctypes.data),
                allow_not_converged=not strict)
         return (wrench, tau, status) if torques else (wrench, status)
+
+    def _states_call(self, fn, states, mask, shift, torques, strict, out, dt_mpc):
+        from .scenarios import STATE_DTYPE
+
+        if states.dtype != STATE_DTYPE or not states.flags.c_contiguous:
+            states = np.ascontiguousarray(states, dtype=STATE_DTYPE)
+        B = states.shape[0]
+        if out is not None:
+            wrench, status = out
+            assert wrench.dtype == np.float64 and wrench.shape == (B, 12 * self.horizon) and wrench.flags.c_contiguous
+            assert status.dtype == np.int32 and status.shape == (B,)
+        else:
+            wrench = np.zeros((B, 12 * self.horizon), dtype=np.float64)
+            status = np.zeros(B, dtype=np.int32)
+        tau = np.zeros((B, 10), dtype=np.float64) if torques else None
+        if shift is not None:
+            shift = np.ascontiguousarray(shift, dtype=np.int32)
+            assert shift.shape == (B,)
+        args = [self._h, states.ctypes.data, B]
+        if mask is not None:
+            mask = np.ascontiguousarray(np.asarray(mask) != 0).view(np.uint8)
+            assert mask.shape == (B,)
+            args.append(mask.ctypes.data)
+        _check(fn(*args, dt_mpc, wrench.ctypes.data, tau.ctypes.data if torques else None, status.ctypes.data,
+                  shift.ctypes.data if shift is not None else None),
+               allow_not_converged=not strict)
+        return (wrench, tau, status) if torques else (wrench, status)
+
+    def solve_batch_states_warm(self, states: np.ndarray, shift=None, torques: bool = False, strict: bool = True, out=None,
+                                dt_mpc: float = 0.04):
+        """solve_batch_states warm-started from each robot's working set of its last warm call (hmpc_solve_batch_states_warm).
+        `shift` int32 [B]: steps robot i's horizon moved since then (None: all 1; 0: same horizon; < 0: no history).
+        In place when the states, wrench and status arrays are pinned (pin()).  -> (wrench, status), or (wrench, tau, status)
+        with torques=True."""
+        return self._states_call(lib().hmpc_solve_batch_states_warm, states, None, shift, torques, strict, out, dt_mpc)
+
+    def solve_batch_states_masked(self, states: np.ndarray, mask, shift=None, torques: bool = False, strict: bool = True,
+                                  out=None, dt_mpc: float = 0.04):
+        """solve_batch_states_warm of the robots with mask[i] != 0 only (hmpc_solve_batch_states_masked): `mask` bool or uint8
+        [B], `shift` int32 [B] read for listed robots only (None: 1 each).  Only listed rows of the results are written.  With
+        out=None the arrays are new and unlisted rows hold zeros (a status of 0 there means "not solved", not "optimal");
+        with `out=(wrench, status)` they keep what the caller's arrays held.  strict: raise when a listed robot did not
+        converge.  -> (wrench, status), or (wrench, tau, status) with torques=True."""
+        return self._states_call(lib().hmpc_solve_batch_states_masked, states, mask, shift, torques, strict, out, dt_mpc)
 
     def prepare_device(self, d_states, B: int, d_records, stream=None, dt_mpc: float = 0.04) -> None:
         """Row f-1 on device-resident data: torch uint8 [B,352] states -> packed records [B,stride].
@@ -482,6 +536,20 @@ class BatchedMPC:
         _check(lib().hmpc_solve_device_masked(self._h, d_records.data_ptr(), B, d_mask.data_ptr(), d_wrench.data_ptr(),
                                               d_status.data_ptr(), d_tau.data_ptr() if d_tau is not None else None,
                                               d_shift.data_ptr() if d_shift is not None else None, ctypes.c_void_p(st)))
+
+    def solve_states_device_masked(self, d_states, B: int, d_mask, d_records, d_wrench, d_status, d_tau=None, d_shift=None,
+                                   stream=None, dt_mpc: float = 0.04) -> None:
+        """solve_device_masked on robot states (hmpc_solve_states_device_masked): one chain prepares the listed robots'
+        records into `d_records` (uint8 [B,stride]; unlisted rows keep their bytes) and solves them.  `d_states` torch uint8
+        [B,352] on the GPU, the other arguments as in solve_device_masked.  Capturable in a CUDA graph: a replay prepares
+        and solves the robots the captured mask lists from the states the captured tensor holds when it runs."""
+        import torch
+
+        st = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        _check(lib().hmpc_solve_states_device_masked(self._h, d_states.data_ptr(), B, d_mask.data_ptr(), dt_mpc,
+                                                     d_records.data_ptr(), d_wrench.data_ptr(), d_status.data_ptr(),
+                                                     d_tau.data_ptr() if d_tau is not None else None,
+                                                     d_shift.data_ptr() if d_shift is not None else None, ctypes.c_void_p(st)))
 
     def assemble_device(self, d_records, B: int, stream=None) -> dict:
         """Parity hook: un-reduced fp32 QP data of B packed records (torch tensors on the GPU)."""

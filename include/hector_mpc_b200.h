@@ -193,7 +193,10 @@ HMPC_EXTERNC int hmpc_unpin_host_buffer(hmpc_ctx* ctx, void* ptr);
  * offsets + fmod, foot positions r, weights, the 12 x horizon reference trajectory, double -> float narrowing:
  * ConvexMPCLocomotion.cpp:283-406 + convexMPC_interface.cpp:87-99) with one GPU thread per robot, so a tick moves
  * 352 bytes per robot to the device instead of a 720-byte record.  hmpc_solve_batch_states = H2D of the states +
- * hmpc_prepare_device + the solve of hmpc_solve_batch_ex. */
+ * hmpc_prepare_device + the solve of hmpc_solve_batch_ex; with the states, wrench_out and status pinned
+ * (hmpc_pin_host_buffer) it runs in place, as hmpc_solve_batch does: the same solve, with the wrenches stored as the
+ * solver's doubles rather than their float rounding, as in hmpc_solve_batch's in-place mode.  The warm and masked calls on
+ * states follow hmpc_solve_batch_masked below. */
 struct hmpc_state_t
 {
   double position[3];              /* seResult.position */
@@ -278,6 +281,23 @@ HMPC_EXTERNC int hmpc_solve_device_masked(hmpc_ctx* ctx, const void* d_records, 
                                           float* d_wrench, int* d_status, float* d_tau, const int* d_shift, void* stream);
 HMPC_EXTERNC int hmpc_solve_batch_masked(hmpc_ctx* ctx, const struct update_data_t* in, int B, const unsigned char* mask,
                                          double* wrench_out, double* tau_out, int* status, const int* shift);
+/* The same calls with robot states (hmpc_state_t) in: the data preparation of hmpc_prepare_device, then the solve.
+ *   hmpc_solve_states_device_masked: one chain on `stream`, the selection kernel, then the preparation of the listed robots
+ *                             only, then the solve of hmpc_solve_device_masked.  d_records [B][hmpc_record_bytes] (16-byte
+ *                             aligned) receives the listed robots' records, what the solver saw; unlisted rows keep their
+ *                             bytes.  Capturable, as hmpc_solve_device_masked.
+ *   hmpc_solve_batch_states_warm / _masked: hmpc_solve_batch_warm / _masked on states, in all three host-buffer modes.
+ * Like hmpc_solve_batch_states, these calls run in place when the states array, wrench_out and status (if given) lie in
+ * pinned ranges (hmpc_pin_host_buffer): the preparation kernel reads the states where they lie, the records stay in the
+ * context, and double wrenches and status words are written straight into the caller's arrays. */
+HMPC_EXTERNC int hmpc_solve_states_device_masked(hmpc_ctx* ctx, const struct hmpc_state_t* d_states, int B,
+                                                 const unsigned char* d_mask, double dtMPC, void* d_records, float* d_wrench,
+                                                 int* d_status, float* d_tau, const int* d_shift, void* stream);
+HMPC_EXTERNC int hmpc_solve_batch_states_warm(hmpc_ctx* ctx, const struct hmpc_state_t* in, int B, double dtMPC,
+                                              double* wrench_out, double* tau_out, int* status, const int* shift);
+HMPC_EXTERNC int hmpc_solve_batch_states_masked(hmpc_ctx* ctx, const struct hmpc_state_t* in, int B, const unsigned char* mask,
+                                                double dtMPC, double* wrench_out, double* tau_out, int* status,
+                                                const int* shift);
 /* The reference boundary warm-started: after hmpc_reference_set_warm_start(1), every update_problem_data proposes the
  * previous call's working set moved one step (a hmpc_solve_batch_warm with shift NULL on the one-robot context).
  * setup_problem with another dt, f_max or horizon forgets it.  Default 0: every tick a cold start, like the reference. */
@@ -338,7 +358,8 @@ HMPC_EXTERNC int hmpc_swing_device(hmpc_ctx* ctx, const struct hmpc_state_t* d_s
 
 /* CUDA graphs.  The device-resident calls can be recorded into a CUDA graph by stream capture (cudaStreamBeginCapture,
  * torch.cuda.graph, ...) on the stream they are given: hmpc_solve_device, hmpc_solve_device_ex, hmpc_solve_device_warm,
- * hmpc_solve_device_masked, hmpc_prepare_device, hmpc_rollout_device, hmpc_swing_device and hmpc_reset_warm_start.  Each
+ * hmpc_solve_device_masked, hmpc_solve_states_device_masked, hmpc_prepare_device, hmpc_rollout_device, hmpc_swing_device
+ * and hmpc_reset_warm_start.  Each
  * launch of the graph gives the results an eager call on the same inputs gives, bit for bit.
  *   - A replay is a real call.  A captured warm solve proposes and records working sets, a captured rollout advances
  *     d_states and d_loop, a captured hmpc_reset_warm_start clears the working sets, every time the graph is launched.
@@ -349,7 +370,8 @@ HMPC_EXTERNC int hmpc_swing_device(hmpc_ctx* ctx, const struct hmpc_state_t* d_s
  *   - A graph must not be launched after hmpc_destroy of its context.
  *   - A call that returns an error while its stream is capturing may have recorded part of its work: end the capture
  *     and discard the graph.  Argument errors are found before anything is enqueued.
- * The host-buffer calls (hmpc_solve_batch, _ex, _warm, _masked, _states, hmpc_solve_batch_sharded) and the reference boundary
+ * The host-buffer calls (hmpc_solve_batch, _ex, _warm, _masked, _states, _states_warm, _states_masked,
+ * hmpc_solve_batch_sharded) and the reference boundary
  * (update_problem_data) wait for their own streams and cannot be captured. */
 
 /* Robots beyond the conditioning limit (INTEGRATION.md).  The fp64 sweep inversion of the solve is accurate up to a scaled
