@@ -6,6 +6,7 @@
 #include <dlfcn.h>
 #include <unistd.h>
 
+#include <algorithm>
 #include <chrono>
 #include <cstddef>
 #include <cstdint>
@@ -116,7 +117,16 @@ class HostPool {
   std::atomic<int> pending_{0};
 };
 
-constexpr int NCHUNK = 4;  // the host-buffer path pipelines pack / H2D / solve / D2H over this many chunks
+constexpr int NCHUNK = 4;  // the host-buffer path pipelines pack / H2D / solve / D2H over this many chunks at most
+
+// The slots of d_cls: eager device-resident chains use one, chains recorded into a CUDA graph the other (enqueue_solve).
+constexpr int EAGER_SLOT = 0, CAPTURE_SLOT = 1, CLS_SLOTS = 2;
+static_assert(CAPTURE_SLOT < CLS_SLOTS, "d_cls holds CLS_SLOTS slots");
+
+// A view of rows [b0, b0 + nb) of the context's result staging (d_out, h_out).  The chunk of those rows starts at byte
+// b0 * hmpc_ctx::row_bytes() and holds [nb][12N] float wrenches, then [nb] status words, then [nb][10] float torques.
+// tau is null in a view without torques; bytes counts wrenches, status words and (if in the view) torques.
+struct ResultRows { float* wrench; int* status; float* tau; size_t bytes; };
 
 using hmpc::ClassCfg;
 
@@ -132,14 +142,13 @@ struct hmpc_ctx {
   ClassCfg ref{};
   int* d_ref = nullptr;            // host-buffer path: [NCHUNK][1 + max_batch] refinement list length + list
   unsigned char* d_rec = nullptr;
-  unsigned char* d_out = nullptr;  // host-buffer path: per chunk [wrench floats | status ints], contiguous
+  unsigned char* d_out = nullptr;  // host-buffer path: result staging (rows())
   int* d_status = nullptr;         // scratch status (assembly hook)
-  int* d_counts = nullptr;         // [NCHUNK][4] class list lengths (assembly hook)
+  int* d_counts = nullptr;         // [4] class list lengths (assembly hook)
   int* d_lists = nullptr;          // [NCHUNK][host_lists_ints] class lists (host-built, host-buffer path)
-  int* d_cls = nullptr;            // [NCHUNK][ClassSlot::cls_slot_ints] class-list lengths and lists (device-resident
-                                   // path; slot 0: eager chains, slot 1: chains recorded into a CUDA graph)
+  int* d_cls = nullptr;            // [CLS_SLOTS][ClassSlot::cls_slot_ints] class-list lengths and lists (device-resident path)
   unsigned char* h_mask = nullptr; // pinned [max_batch]: the mask of hmpc_solve_batch_masked, read mapped by the in-place mode
-  unsigned tick[NCHUNK] = {0, 0, 0, 0};  // eager calls per slot: parity of the list lengths in use
+  unsigned eager_calls = 0;        // eager device-resident chains so far: parity of the list lengths in use
   unsigned char* h_rec = nullptr;  // pinned
   unsigned char* h_out = nullptr;  // pinned mirror of d_out
   unsigned char* d_states = nullptr;  // hmpc_state_t staging of hmpc_solve_batch_states (row f-1)
@@ -152,9 +161,7 @@ struct hmpc_ctx {
   void* nccl = nullptr;            // ncclComm_t
   int shard_rank = 0, shard_world = 1;
   float* shard_buf[2] = {nullptr, nullptr};   // [max_batch][12N] this rank's results of tick t / t+1
-  float* shard_out = nullptr;      // where the kernels of the current sharded tick also store float results (else null)
   unsigned shard_tick = 0;
-  bool shard_used = false;         // the in-place chain stored this tick's floats (else the staged path ran)
   cudaStream_t gstream = nullptr;  // the gather runs here, behind `solved`, beside the next tick
   cudaEvent_t solved = nullptr, gathered[2] = {nullptr, nullptr};
   int* d_ws = nullptr;             // [max_batch][WS_STATE_INTS] working sets of the previous tick (closed-loop warm start)
@@ -173,6 +180,14 @@ struct hmpc_ctx {
     for (const Pin& r : pins)
       if (q >= r.base && q + bytes <= r.base + r.bytes) return true;
     return false;
+  }
+  size_t row_bytes() const { return (size_t)12 * horizon * 4 + 4 + 40; }  // one robot's results in d_out / h_out
+  ResultRows rows(unsigned char* base, int b0, int nb, bool tau = true) const
+  {
+    const size_t nw = (size_t)12 * horizon;
+    unsigned char* p = base + (size_t)b0 * row_bytes();
+    return {reinterpret_cast<float*>(p), reinterpret_cast<int*>(p + (size_t)nb * nw * 4),
+            tau ? reinterpret_cast<float*>(p + (size_t)nb * (nw * 4 + 4)) : nullptr, (size_t)nb * (nw * 4 + 4 + (tau ? 40 : 0))};
   }
 };
 
@@ -395,43 +410,6 @@ HMPC_EXTERNC int hmpc_shard_init(hmpc_ctx* c, int rank, int world, const void* i
   return HMPC_OK;
 }
 
-HMPC_EXTERNC int hmpc_solve_batch_sharded(hmpc_ctx* c, const update_data_t* in_local, int B_local, double* wrench_local,
-                                          int* status_local, float* d_all)
-{
-  if (!c || !c->nccl) { g_err = "hmpc_solve_batch_sharded: call hmpc_shard_init first"; return HMPC_ERR_ARG; }
-  if (B_local < 1 || B_local > c->max_batch) { g_err = "hmpc_solve_batch_sharded: every rank needs 1 <= B_local <= capacity"; return HMPC_ERR_ARG; }
-  CK(cudaSetDevice(c->device));
-  const int par = (int)(c->shard_tick++ & 1u);
-  const size_t nw = (size_t)12 * c->horizon;
-  if (d_all) {
-    // this tick's kernels also leave float results in shard_buf[par]; the gather that last read it (two ticks ago)
-    // must be done before they overwrite it — a stream-side wait, the host does not block
-    CK(cudaStreamWaitEvent(c->stream, c->gathered[par], 0));
-    c->shard_out = c->shard_buf[par];
-  }
-  const int rc = hmpc_solve_batch(c, in_local, B_local, wrench_local, status_local);
-  const bool staged = d_all && c->shard_out && !c->shard_used;
-  c->shard_out = nullptr;
-  if (rc != HMPC_OK && rc != HMPC_ERR_NOT_CONVERGED) return rc;
-  if (d_all) {
-    if (staged) {
-      // the staged host path did not run the in-place chain: put the float results on the device for the gather
-      std::vector<float> tmp((size_t)B_local * nw);
-      for (size_t i = 0; i < tmp.size(); i++) tmp[i] = (float)wrench_local[i];
-      CK(cudaMemcpyAsync(c->shard_buf[par], tmp.data(), tmp.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-      CK(cudaStreamSynchronize(c->stream));
-      CK(cudaEventRecord(c->solved, c->stream));
-    }
-    c->shard_used = false;
-    // the path's ONE collective: every rank's slice of float wrenches to every device, beside the next tick
-    CK(cudaStreamWaitEvent(c->gstream, c->solved, 0));
-    if (nccl_fail(g_nccl.AllGather(c->shard_buf[par], d_all, (size_t)B_local * nw, /* ncclFloat32 */ 7, c->nccl, c->gstream), "ncclAllGather"))
-      return HMPC_ERR_CUDA;
-    CK(cudaEventRecord(c->gathered[par], c->gstream));
-  }
-  return rc;
-}
-
 HMPC_EXTERNC int hmpc_shard_wait(hmpc_ctx* c)
 {
   if (!c || !c->nccl) { g_err = "hmpc_shard_wait: call hmpc_shard_init first"; return HMPC_ERR_ARG; }
@@ -497,28 +475,27 @@ HMPC_EXTERNC hmpc_ctx* hmpc_create(int max_batch, int horizon, int device)
   }
   if (!bad) {
     c->sm_count = prop.multiProcessorCount;
-    const size_t nw = (size_t)12 * horizon;
     bad = cuda_fail(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking), "cudaStreamCreate") ||
           cuda_fail(cudaStreamCreateWithFlags(&c->xstream[0], cudaStreamNonBlocking), "cudaStreamCreate") ||
           cuda_fail(cudaStreamCreateWithFlags(&c->xstream[1], cudaStreamNonBlocking), "cudaStreamCreate") ||
           cuda_fail(cudaStreamCreateWithFlags(&c->xstream[2], cudaStreamNonBlocking), "cudaStreamCreate") ||
           cuda_fail(cudaMalloc(&c->d_rec, (size_t)max_batch * c->rec_stride), "cudaMalloc records") ||
-          cuda_fail(cudaMalloc(&c->d_out, (size_t)max_batch * (nw * 4 + 4 + 40)), "cudaMalloc results") ||
-          cuda_fail(cudaMalloc(&c->d_counts, NCHUNK * 4 * sizeof(int)), "cudaMalloc counts") ||
+          cuda_fail(cudaMalloc(&c->d_out, (size_t)max_batch * c->row_bytes()), "cudaMalloc results") ||
+          cuda_fail(cudaMalloc(&c->d_counts, 4 * sizeof(int)), "cudaMalloc counts") ||
           cuda_fail(cudaMalloc(&c->d_lists, (size_t)NCHUNK * hmpc::host_lists_ints(max_batch) * sizeof(int)), "cudaMalloc lists") ||
           cuda_fail(cudaMalloc(&c->d_ws, (size_t)max_batch * hmpc::WS_STATE_INTS * sizeof(int)), "cudaMalloc working sets") ||
           cuda_fail(cudaMemset(c->d_ws, 0, (size_t)max_batch * hmpc::WS_STATE_INTS * sizeof(int)), "cudaMemset working sets") ||
           cuda_fail(cudaMalloc(&c->d_shift, (size_t)max_batch * sizeof(int)), "cudaMalloc shifts") ||
           cuda_fail(cudaMallocHost(&c->h_shift, (size_t)max_batch * sizeof(int)), "cudaMallocHost shifts") ||
           cuda_fail(cudaMallocHost(&c->h_mask, (size_t)max_batch), "cudaMallocHost mask") ||
-          cuda_fail(cudaMalloc(&c->d_cls, (size_t)NCHUNK * hmpc::ClassSlot::cls_slot_ints(max_batch) * sizeof(int)), "cudaMalloc class lists") ||
-          cuda_fail(cudaMemset(c->d_cls, 0, (size_t)NCHUNK * hmpc::ClassSlot::cls_slot_ints(max_batch) * sizeof(int)), "cudaMemset class lists") ||
+          cuda_fail(cudaMalloc(&c->d_cls, (size_t)CLS_SLOTS * hmpc::ClassSlot::cls_slot_ints(max_batch) * sizeof(int)), "cudaMalloc class lists") ||
+          cuda_fail(cudaMemset(c->d_cls, 0, (size_t)CLS_SLOTS * hmpc::ClassSlot::cls_slot_ints(max_batch) * sizeof(int)), "cudaMemset class lists") ||
           cuda_fail(cudaMalloc(&c->d_ref, (size_t)NCHUNK * (1 + (size_t)max_batch) * sizeof(int)), "cudaMalloc refinement lists") ||
           cuda_fail(cudaMalloc(&c->d_status, (size_t)max_batch * 4), "cudaMalloc status") ||
           cuda_fail(cudaMalloc(&c->d_states, (size_t)max_batch * sizeof(hmpc_state_t)), "cudaMalloc states") ||
           cuda_fail(cudaMallocHost(&c->h_states, (size_t)max_batch * sizeof(hmpc_state_t)), "cudaMallocHost states") ||
           cuda_fail(cudaMallocHost(&c->h_rec, (size_t)max_batch * c->rec_stride), "cudaMallocHost records") ||
-          cuda_fail(cudaMallocHost(&c->h_out, (size_t)max_batch * (nw * 4 + 4 + 40)), "cudaMallocHost results") ||
+          cuda_fail(cudaMallocHost(&c->h_out, (size_t)max_batch * c->row_bytes()), "cudaMallocHost results") ||
           cuda_fail(cudaMallocHost(&c->h_cls, (size_t)NCHUNK * hmpc::host_lists_ints(max_batch) * sizeof(int)), "cudaMallocHost lists") ||
           build_classes(c) != HMPC_OK;
   }
@@ -560,9 +537,6 @@ HMPC_EXTERNC int hmpc_set_problem(hmpc_ctx* c, const problem_setup* s)
 }
 
 namespace {
-// The slot of d_cls whose list lengths a chain recorded into a CUDA graph uses.  Eager chains use slot 0.
-constexpr int CAPTURE_SLOT = 1;
-static_assert(CAPTURE_SLOT < NCHUNK, "d_cls holds NCHUNK slots");
 // The device-resident chain: one launch per class, all enqueued on `st`; with io.mask (device-readable [B]) the selection
 // kernel first, and with io.states the preparation of the robots class 0 runs over (hmpc_chain.h).  No classification kernel: the class-0 launch runs over every instance (or, in a masked call, over the list
 // the selection kernel built from the mask) and hands the ones with more stance blocks than it holds to class 1's list.
@@ -577,9 +551,9 @@ int enqueue_solve(hmpc_ctx* c, const hmpc::SolveIO& io, cudaStream_t st)
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   CK(cudaStreamIsCapturing(st, &cap));
   const bool capturing = cap != cudaStreamCaptureStatusNone;
-  const int slot = capturing ? CAPTURE_SLOT : 0;
+  const int slot = capturing ? CAPTURE_SLOT : EAGER_SLOT;
   const hmpc::ClassSlot s{c->d_cls + (size_t)slot * hmpc::ClassSlot::cls_slot_ints(c->max_batch), c->max_batch,
-                          capturing ? 0 : (int)(c->tick[slot]++ & 1u)};
+                          capturing ? 0 : (int)(c->eager_calls++ & 1u)};
   if (capturing) CK(cudaMemsetAsync(s.base, 0, hmpc::ClassSlot::HEAD_INTS * sizeof(int), st));
   const hmpc::ChainLists lists = hmpc::slot_lists(s, io.mask != nullptr, c->cfg.refine);
   const bool pdl = pdl_enabled();
@@ -615,31 +589,26 @@ hmpc::SolveIO device_call(const hmpc_ctx* c, const void* d_records, int B, float
   return io;
 }
 
-// Host-buffer path: the host has the contact tables in hand while it packs, so it builds the class lists itself
+// Host-buffer path, staged: the host has the contact tables in hand while it packs, so it builds the class lists itself
 // (hmpc::classify_host) and launches only the non-empty classes — no classification kernel, no empty launches.
 // Working-set overflow cannot escalate here (enqueue_overflow_retry), nor can the refinement class run (enqueue_refine_retry).
+// A chunk is robots [b0, b0 + nb) on stream st with their device views (io), their host-built class lists (lists; d_lists:
+// the device copy) and their refinement list (ref; null while refinement is off).
+struct Chunk { int b0, nb; cudaStream_t st; hmpc::SolveIO io; int *lists, *d_lists, *ref; };
 
-// the host-built lists of chunk `k` at `block` (device-readable) and the chunk's refinement list while refinement is on
-hmpc::ChainLists chunk_lists(const hmpc_ctx* c, int k, int* block, bool escalate)
+int enqueue_solve_hostlists(hmpc_ctx* c, const Chunk& ch, bool zero_copy)
 {
-  int* ref = c->d_ref + (size_t)k * (1 + (size_t)c->max_batch);
-  return hmpc::host_lists(block, c->max_batch, c->cfg.refine ? ref : nullptr, escalate);
-}
-
-int enqueue_solve_hostlists(hmpc_ctx* c, const hmpc::SolveIO& io, int* h_block, cudaStream_t st, int k, bool zero_copy)
-{
-  int* d_block = zero_copy ? h_block : c->d_lists + (size_t)k * hmpc::host_lists_ints(c->max_batch);
-  const int n0 = h_block[0], n1 = h_block[1];
-  if (!zero_copy) {  // else pinned + mapped: the kernels read the lists over PCIe, no copy launch
-    // counts + class-0 list (+ class-1 list when it is not empty) in one copy
-    const size_t ints = n1 > 0 ? hmpc::host_list(h_block, c->max_batch, 1) - h_block + n1 : hmpc::HOST_LIST_HEAD + n0;
-    CK(cudaMemcpyAsync(d_block, h_block, ints * sizeof(int), cudaMemcpyHostToDevice, st));
+  int* h_block = ch.lists;
+  int* d_block = zero_copy ? h_block : ch.d_lists;  // zero-copy: pinned + mapped, the kernels read the lists over PCIe
+  if (!zero_copy) {  // counts + class-0 list (+ class-1 list when it is not empty) in one copy
+    const size_t ints = h_block[1] > 0 ? hmpc::host_list(h_block, c->max_batch, 1) - h_block + h_block[1] : hmpc::HOST_LIST_HEAD + h_block[0];
+    CK(cudaMemcpyAsync(d_block, h_block, ints * sizeof(int), cudaMemcpyHostToDevice, ch.st));
   }
-  const hmpc::ChainLists lists = chunk_lists(c, k, d_block, false);
-  if (c->cfg.refine) CK(cudaMemsetAsync(lists.ref_count, 0, sizeof(int), st));
+  const hmpc::ChainLists lists = hmpc::host_lists(d_block, c->max_batch, ch.ref, false);
+  if (ch.ref) CK(cudaMemsetAsync(lists.ref_count, 0, sizeof(int), ch.st));
   for (int i = 0; i < 2; i++)
     if (h_block[i] > 0)
-      if (int rc = launch_class(c, i, io, lists, h_block[i], st)) return rc;
+      if (int rc = launch_class(c, i, ch.io, lists, h_block[i], ch.st)) return rc;
   return HMPC_OK;
 }
 
@@ -647,12 +616,12 @@ int enqueue_solve_hostlists(hmpc_ctx* c, const hmpc::SolveIO& io, int* h_block, 
 // solved again, from where the device-resident chain would have taken them: class 0's by class 1, class 1's by class 2,
 // with escalation from the one to the other.  The rest of the chunk keeps its results and its recorded working sets, and an
 // instance that overflowed kept its proposal (the kernel does not record a set for it), so results, statuses and working
-// sets are those of the device-resident path.  `h_block` holds the chunk's class lists and is reused for the retry's.
+// sets are those of the device-resident path.  The chunk's class lists are reused for the retry's.
 // `mask` (the chunk's, host) or NULL: the status words of robots it does not list are stale and are not looked at.
-int enqueue_overflow_retry(hmpc_ctx* c, const hmpc::SolveIO& io, int* h_block, const int* h_status, cudaStream_t st, int k,
-                           const unsigned char* mask)
+int enqueue_overflow_retry(hmpc_ctx* c, const Chunk& ch, const int* h_status, const unsigned char* mask)
 {
-  const int mb = c->max_batch, nb = io.batch;
+  const int mb = c->max_batch, nb = ch.nb;
+  int* h_block = ch.lists;
   std::vector<char> was_cls1(nb, 0);
   for (int j = 0; j < h_block[1]; j++) was_cls1[hmpc::host_list(h_block, mb, 1)[j]] = 1;
   int n[3] = {0, 0, 0};
@@ -665,13 +634,12 @@ int enqueue_overflow_retry(hmpc_ctx* c, const hmpc::SolveIO& io, int* h_block, c
   h_block[1] = n[1];
   h_block[2] = n[2];
   h_block[3] = 0;
-  int* d_block = c->d_lists + (size_t)k * hmpc::host_lists_ints(mb);
-  CK(cudaMemcpyAsync(d_block, h_block, (hmpc::host_list(h_block, mb, 2) - h_block + n[2]) * sizeof(int), cudaMemcpyHostToDevice, st));
-  const hmpc::ChainLists lists = chunk_lists(c, k, d_block, true);
+  CK(cudaMemcpyAsync(ch.d_lists, h_block, (hmpc::host_list(h_block, mb, 2) - h_block + n[2]) * sizeof(int), cudaMemcpyHostToDevice, ch.st));
+  const hmpc::ChainLists lists = hmpc::host_lists(ch.d_lists, mb, ch.ref, true);
   for (int i = 1; i < c->ncls; i++) {
     const int cnt = (i == 1) ? n[1] : n[1] + n[2];  // class 2's list grows by class 1's escalations
     if (cnt > 0)
-      if (int rc = launch_class(c, i, io, lists, cnt, st)) return rc;
+      if (int rc = launch_class(c, i, ch.io, lists, cnt, ch.st)) return rc;
   }
   return HMPC_OK;
 }
@@ -679,10 +647,9 @@ int enqueue_overflow_retry(hmpc_ctx* c, const hmpc::SolveIO& io, int* h_block, c
 // Refinement in a host-list launch: the kernels pushed the instances beyond the conditioning limit to the chunk's refinement
 // list (device memory), and the refinement class solves them as it does at the end of the device-resident chain.  Called
 // when refinement is on and a status of the chunk has code 4 (a non-positive pivot is not on the list).
-int enqueue_refine_retry(hmpc_ctx* c, const hmpc::SolveIO& io, cudaStream_t st, int k)
+int enqueue_refine_retry(hmpc_ctx* c, const Chunk& ch)
 {
-  int* d_block = c->d_lists + (size_t)k * hmpc::host_lists_ints(c->max_batch);
-  return launch_class(c, hmpc::REFINE_CLASS, io, chunk_lists(c, k, d_block, false), io.batch, st);
+  return launch_class(c, hmpc::REFINE_CLASS, ch.io, hmpc::host_lists(ch.d_lists, c->max_batch, ch.ref, false), ch.nb, ch.st);
 }
 }  // namespace
 
@@ -787,35 +754,6 @@ HMPC_EXTERNC int hmpc_assemble_device(hmpc_ctx* c, const void* d_records, int B,
   hmpc::ChainLists lists;
   lists.counts = c->d_counts;
   return launch_class(c, c->ncls - 1, io, lists, B, static_cast<cudaStream_t>(stream));
-}
-
-static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_state_t* sin, int B, double* wrench_out,
-                            double* tau_out, int* status, double dtMPC = 0.0, bool warm = false, const int* shift = nullptr,
-                            const unsigned char* mask = nullptr);
-
-HMPC_EXTERNC int hmpc_solve_batch(hmpc_ctx* c, const update_data_t* in, int B, double* wrench_out, int* status)
-{
-  return solve_batch_impl(c, in, nullptr, B, wrench_out, nullptr, status);
-}
-
-HMPC_EXTERNC int hmpc_solve_batch_ex(hmpc_ctx* c, const update_data_t* in, int B, double* wrench_out, double* tau_out,
-                                     int* status)
-{
-  return solve_batch_impl(c, in, nullptr, B, wrench_out, tau_out, status);
-}
-
-HMPC_EXTERNC int hmpc_solve_batch_warm(hmpc_ctx* c, const update_data_t* in, int B, double* wrench_out, double* tau_out,
-                                       int* status, const int* shift)
-{
-  if (!in) { g_err = "hmpc_solve_batch_warm: bad argument (null records)"; return HMPC_ERR_ARG; }
-  return solve_batch_impl(c, in, nullptr, B, wrench_out, tau_out, status, 0.0, true, shift);
-}
-
-HMPC_EXTERNC int hmpc_solve_batch_masked(hmpc_ctx* c, const update_data_t* in, int B, const unsigned char* mask, double* wrench_out,
-                                         double* tau_out, int* status, const int* shift)
-{
-  if (!in || !mask) { g_err = "hmpc_solve_batch_masked: bad argument (null records or mask)"; return HMPC_ERR_ARG; }
-  return solve_batch_impl(c, in, nullptr, B, wrench_out, tau_out, status, 0.0, true, shift, mask);
 }
 
 static_assert(sizeof(hmpc_state_t) == 352 && offsetof(hmpc_state_t, gait) == 39 * 8, "hmpc_state_t layout (hmpc_prepare_kernel)");
@@ -928,19 +866,18 @@ HMPC_EXTERNC int hmpc_rollout_device(hmpc_ctx* c, hmpc_state_t* d_states, hmpc_r
   if (B == 0) return HMPC_OK;
   CK(cudaSetDevice(c->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const size_t nw = (size_t)12 * c->horizon;
-  float* dw = reinterpret_cast<float*>(c->d_out);  // the context's own result area is the loop's scratch
-  int* ds = reinterpret_cast<int*>(c->d_out + (size_t)c->max_batch * nw * 4);
+  const ResultRows scratch = c->rows(c->d_out, 0, c->max_batch);  // the context's own result area is the loop's scratch
   for (int t = 0; t < ticks; t++) {
     int rc = hmpc_prepare_device(c, d_states, B, dtMPC, c->d_rec, st);
     if (rc != HMPC_OK) return rc;
     if (d_record_log)
       CK(cudaMemcpyAsync(static_cast<unsigned char*>(d_record_log) + (size_t)t * B * c->rec_stride, c->d_rec,
                          (size_t)B * c->rec_stride, cudaMemcpyDeviceToDevice, st));
-    rc = enqueue_solve(c, device_call(c, c->d_rec, B, dw, ds, nullptr, true), st);
+    rc = enqueue_solve(c, device_call(c, c->d_rec, B, scratch.wrench, scratch.status, nullptr, true), st);
     if (rc != HMPC_OK) return rc;
     hmpc::hmpc_advance_kernel<<<(B + 63) / 64, 64, 0, st>>>(reinterpret_cast<unsigned char*>(d_states),
-                                                            reinterpret_cast<unsigned char*>(d_loop), B, c->horizon, dtMPC, dw, ds,
+                                                            reinterpret_cast<unsigned char*>(d_loop), B, c->horizon, dtMPC,
+                                                            scratch.wrench, scratch.status,
                                                             d_wrench_log ? d_wrench_log + (size_t)t * B * 12 : nullptr);
     CK(cudaGetLastError());
   }
@@ -971,244 +908,304 @@ HMPC_EXTERNC int hmpc_swing_device(hmpc_ctx* c, const hmpc_state_t* d_states, co
   return HMPC_OK;
 }
 
-HMPC_EXTERNC int hmpc_solve_batch_states(hmpc_ctx* c, const hmpc_state_t* in, int B, double dtMPC, double* wrench_out,
-                                         double* tau_out, int* status)
+// ---------------------------------------------------------------------------------------------------
+// host-buffer calls (hmpc_solve_batch and its variants): the caller's arrays are in host memory
+// ---------------------------------------------------------------------------------------------------
+namespace {
+// What one host-buffer call asks for.  Unused pointers stay null.
+struct HostCall {
+  HostCall(const update_data_t* in, int B, double* w, double* t, int* st) : records(in), batch(B), wrench(w), tau(t), status(st) {}
+  HostCall(const hmpc_state_t* in, int B, double dt, double* w, double* t, int* st)
+      : states(in), dt_mpc(dt), batch(B), wrench(w), tau(t), status(st) {}
+  HostCall& warm_start(const int* s, const unsigned char* m = nullptr) { warm = true, shift = s, mask = m; return *this; }
+  const update_data_t* records = nullptr;  // the reference's records in, or
+  const hmpc_state_t* states = nullptr;    // robot states, prepared into records on the device with the MPC step dt_mpc
+  double dt_mpc = 0.0;
+  int batch = 0;
+  double *wrench = nullptr, *tau = nullptr;  // [batch][12N], [batch][10] joint torques
+  int* status = nullptr;                     // [batch]
+  bool warm = false;                         // propose each robot's working set of its last warm call, moved shift[i] steps
+  const int* shift = nullptr;                // (null: one step each)
+  const unsigned char* mask = nullptr;       // [batch]: only robots with mask[i] != 0 are solved and have their rows written
+  float* shard_wrench = nullptr;             // hmpc_solve_batch_sharded in place: the kernels also store float wrenches here,
+  cudaEvent_t shard_solved = nullptr;        // and this event is recorded behind them
+  bool listed(int i) const { return !mask || mask[i] != 0; }
+};
+
+// The mode of a host-buffer call (DESIGN.md §3): in place when the records (or states), the wrenches and the status words
+// (if asked for) lie in buffers registered with hmpc_pin_host_buffer, else staged in chunks (solve_batch_impl).
+constexpr int ZERO_COPY_MAX = 1536;  // above it, packing that overlaps the kernels wins
+
+bool runs_in_place(const hmpc_ctx* c, const HostCall& h)
 {
-  return solve_batch_impl(c, nullptr, in, B, wrench_out, tau_out, status, dtMPC);
+  const size_t B = (size_t)h.batch;
+  const bool in = h.records ? c->pinned(h.records, B * sizeof(update_data_t)) : c->pinned(h.states, B * sizeof(hmpc_state_t));
+  return in && c->pinned(h.wrench, B * 12 * c->horizon * sizeof(double)) && (!h.status || c->pinned(h.status, B * sizeof(int)));
 }
 
-HMPC_EXTERNC int hmpc_solve_batch_states_warm(hmpc_ctx* c, const hmpc_state_t* in, int B, double dtMPC, double* wrench_out,
-                                              double* tau_out, int* status, const int* shift)
+// HMPC_TRACE: microseconds from the start of a staged call to each point, one line on stderr per call
+struct Trace {
+  double t[4 * NCHUNK + 2];
+  int n = 0;
+  void mark()
+  {
+    static const bool on = getenv("HMPC_TRACE") != nullptr;
+    timespec ts;
+    if (on && clock_gettime(CLOCK_MONOTONIC, &ts) == 0) t[n++] = ts.tv_sec * 1e6 + ts.tv_nsec * 1e-3;
+  }
+  void end(int B)
+  {
+    mark();
+    if (n == 0) return;  // (HMPC_TRACE unset)
+    fprintf(stderr, "[hmpc trace] B=%d us since entry:", B);
+    for (int i = 1; i < n; i++) fprintf(stderr, " %.0f", t[i] - t[0]);
+    fprintf(stderr, "  (per chunk: packed, enqueued; then per chunk: synced; end)\n");
+  }
+};
+
+// HMPC_OK when every listed robot of rows [b0, b0 + nb) reached a KKT point (st: their status words)
+int check_converged(const HostCall& h, const int* st, int b0, int nb)
 {
-  if (!in) { g_err = "hmpc_solve_batch_states_warm: bad argument (null states)"; return HMPC_ERR_ARG; }
-  return solve_batch_impl(c, nullptr, in, B, wrench_out, tau_out, status, dtMPC, true, shift);
+  for (int i = 0; i < nb; i++)
+    if (h.listed(b0 + i) && HMPC_STATUS_CODE(st[i]) != 0) {
+      g_err = "hmpc_solve_batch: at least one instance did not reach a KKT point (see status[])";
+      return HMPC_ERR_NOT_CONVERGED;
+    }
+  return HMPC_OK;
 }
 
-HMPC_EXTERNC int hmpc_solve_batch_states_masked(hmpc_ctx* c, const hmpc_state_t* in, int B, const unsigned char* mask,
-                                                double dtMPC, double* wrench_out, double* tau_out, int* status, const int* shift)
+// The device-resident chain on the caller's records (states: prepared into the context's d_rec first), double results
+// stored into the caller's arrays: the call is launches and one synchronize.
+int solve_in_place(hmpc_ctx* c, const HostCall& h, const int* shifts)
 {
-  if (!in || !mask) { g_err = "hmpc_solve_batch_states_masked: bad argument (null states or mask)"; return HMPC_ERR_ARG; }
-  return solve_batch_impl(c, nullptr, in, B, wrench_out, tau_out, status, dtMPC, true, shift, mask);
+  const ResultRows scratch = c->rows(c->h_out, 0, c->max_batch);
+  int* st = h.status ? h.status : scratch.status;
+  float* tau = h.tau ? scratch.tau : nullptr;
+  if (h.mask) memcpy(c->h_mask, h.mask, (size_t)h.batch);  // pinned: the selection kernel reads it mapped
+  hmpc::SolveIO io = device_call(c, h.states ? c->d_rec : nullptr, h.batch, h.shard_wrench, st, tau, h.warm);
+  io.raw = h.records, io.states = h.states, io.dt_mpc = h.dt_mpc;
+  io.wrench64 = h.wrench, io.shifts = shifts, io.mask = h.mask ? c->h_mask : nullptr;
+  if (int rc = enqueue_solve(c, io, c->stream)) return rc;
+  if (h.shard_solved) CK(cudaEventRecord(h.shard_solved, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  if (h.tau)
+    for (int i = 0; i < h.batch; i++)
+      if (h.listed(i))
+        for (int j = 0; j < 10; j++) h.tau[(size_t)i * 10 + j] = (double)tau[(size_t)i * 10 + j];
+  return check_converged(h, st, 0, h.batch);
 }
 
-// mask (hmpc_solve_batch_masked) or NULL: only the robots it lists are solved, and only their rows of wrench_out, tau_out and
-// status are written; the context's staging rows of the others keep stale results, which nothing reads
-static int solve_batch_impl(hmpc_ctx* c, const update_data_t* in, const hmpc_state_t* sin, int B, double* wrench_out,
-                            double* tau_out, int* status, double dtMPC, bool warm, const int* shift, const unsigned char* mask)
+// fn(r0, r1) over rows [b0, b0 + nb), split among the helper threads for large chunks
+template <typename F>
+void over_rows(const hmpc_ctx* c, int b0, int nb, F fn)
 {
-  if (!c || (!in && !sin) || !wrench_out || B < 0 || B > c->max_batch) {
+  if (!c->pool || nb < 128) return fn(b0, b0 + nb);
+  c->pool->parallel([&](int part, int nparts) { fn(b0 + (int)((long long)nb * part / nparts), b0 + (int)((long long)nb * (part + 1) / nparts)); });
+}
+
+// Packs the chunk's records (or stages its states and prepares them on the device), copies them over (copy pipeline),
+// classifies on the host, launches the classes over the host-built lists and copies the results back (copy pipeline).
+int stage_chunk(hmpc_ctx* c, const HostCall& h, bool zc, Chunk& ch, const int* shifts, Trace& tr)
+{
+  const int b0 = ch.b0, nb = ch.nb;
+  const size_t rs = (size_t)c->rec_stride, sb = sizeof(hmpc_state_t);
+  if (h.states) {  // (in a masked call the unlisted robots' records are built too, and not read)
+    memcpy(c->h_states + b0 * sb, h.states + b0, nb * sb);
+    tr.mark();
+    if (!zc) CK(cudaMemcpyAsync(c->d_states + b0 * sb, c->h_states + b0 * sb, nb * sb, cudaMemcpyHostToDevice, ch.st));
+    if (int rc = hmpc_prepare_device(c, reinterpret_cast<const hmpc_state_t*>((zc ? c->h_states : c->d_states) + b0 * sb), nb,
+                                     h.dt_mpc, c->d_rec + b0 * rs, ch.st))
+      return rc;
+  } else {  // every robot of the chunk, or only the listed ones (the kernels read no other record)
+    over_rows(c, b0, nb, [&](int r0, int r1) {
+      if (!h.mask) hmpc_pack_records(h.records + r0, r1 - r0, c->horizon, c->h_rec + r0 * rs);
+      else
+        for (int i = r0; i < r1; i++)
+          if (h.mask[i]) hmpc_pack_records(h.records + i, 1, c->horizon, c->h_rec + i * rs);
+    });
+    tr.mark();
+    if (!zc) CK(cudaMemcpyAsync(c->d_rec + b0 * rs, c->h_rec + b0 * rs, nb * rs, cudaMemcpyHostToDevice, ch.st));
+  }
+  const ResultRows out = c->rows(zc ? c->h_out : c->d_out, b0, nb, h.tau != nullptr);
+  ch.io = device_call(c, ((zc && !h.states) ? c->h_rec : c->d_rec) + b0 * rs, nb, out.wrench, out.status, out.tau, h.warm);
+  if (ch.io.ws) ch.io.ws += (size_t)b0 * hmpc::WS_STATE_INTS;
+  if (shifts && !zc) CK(cudaMemcpyAsync(c->d_shift + b0, shifts + b0, (size_t)nb * sizeof(int), cudaMemcpyHostToDevice, ch.st));
+  if (shifts) ch.io.shifts = (zc ? shifts : c->d_shift) + b0;  // zero-copy: mapped, like the records and lists of this mode
+  hmpc::classify_host(c->horizon, c->cfg.f_max, c->cls[0].nb_hi, h.states ? h.states[b0].gait : h.records[b0].gait,
+                      h.states ? sizeof(hmpc_state_t) : sizeof(update_data_t), nb, ch.lists, c->max_batch, h.mask ? h.mask + b0 : nullptr);
+  if (int rc = enqueue_solve_hostlists(c, ch, zc)) return rc;
+  if (!zc) CK(cudaMemcpyAsync(c->rows(c->h_out, b0, nb).wrench, out.wrench, out.bytes, cudaMemcpyDeviceToHost, ch.st));
+  tr.mark();
+  return HMPC_OK;
+}
+
+// Rows [b0, b0 + nb) of the staged results `r` into the caller's arrays, the listed rows only: wrenches and torques
+// widened to double, status words copied.
+void widen_rows(const hmpc_ctx* c, const HostCall& h, const ResultRows& r, int b0, int nb)
+{
+  const size_t nw = (size_t)12 * c->horizon;
+  over_rows(c, b0, nb, [&](int r0, int r1) {
+    for (int row = r0; row < r1; row++) {
+      if (!h.listed(row)) continue;
+      const size_t i = (size_t)(row - b0);  // the row in the chunk
+      double* w = h.wrench + (size_t)row * nw;
+      const float* src = r.wrench + i * nw;
+      for (size_t e = 0; e < nw; e++) w[e] = (double)src[e];
+      if (h.tau)
+        for (int j = 0; j < 10; j++) h.tau[(size_t)row * 10 + j] = (double)r.tau[i * 10 + j];
+      if (h.status) h.status[row] = r.status[i];
+    }
+  });
+}
+
+// Waits for the chunk, solves again what its host-list launches left (working-set overflow: enqueue_overflow_retry;
+// instances beyond the conditioning limit while refinement is on: enqueue_refine_retry) and widens its results.
+int finish_chunk(hmpc_ctx* c, const HostCall& h, bool zc, Chunk& ch, Trace& tr)
+{
+  CK(cudaStreamSynchronize(ch.st));
+  tr.mark();
+  const ResultRows r = c->rows(c->h_out, ch.b0, ch.nb, h.tau != nullptr);
+  bool overflow = false, not_spd = false;
+  for (int i = 0; i < ch.nb; i++) {
+    overflow |= h.listed(ch.b0 + i) && HMPC_STATUS_CODE(r.status[i]) == hmpc::ST_WS_CAP;
+    not_spd |= h.listed(ch.b0 + i) && HMPC_STATUS_CODE(r.status[i]) == hmpc::ST_NOT_SPD;
+  }
+  const bool refine = c->cfg.refine && not_spd;  // instances handed to the refinement class (on its device-side list)
+  if (overflow || refine) {
+    int rc = overflow ? enqueue_overflow_retry(c, ch, r.status, h.mask ? h.mask + ch.b0 : nullptr) : HMPC_OK;
+    if (rc == HMPC_OK && refine) rc = enqueue_refine_retry(c, ch);
+    if (rc != HMPC_OK) return rc;
+    if (!zc) CK(cudaMemcpyAsync(r.wrench, ch.io.wrench, r.bytes, cudaMemcpyDeviceToHost, ch.st));
+    CK(cudaStreamSynchronize(ch.st));
+  }
+  widen_rows(c, h, r, ch.b0, ch.nb);
+  return HMPC_OK;
+}
+
+// Every host-buffer call.  With a mask the context's staging rows of unlisted robots keep stale results, which nothing reads.
+int solve_batch_impl(hmpc_ctx* c, const HostCall& h)
+{
+  const int B = h.batch;
+  if (!c || (!h.records && !h.states) || !h.wrench || B < 0 || B > c->max_batch) {
     g_err = "hmpc_solve_batch: bad argument (null pointer or batch > capacity)";
     return HMPC_ERR_ARG;
   }
   if (B == 0) return HMPC_OK;
-  if (mask) {
-    bool any = false;
-    for (int i = 0; i < B && !any; i++) any = mask[i] != 0;
-    if (!any) return HMPC_OK;
-  }
-  auto listed = [mask](int i) { return !mask || mask[i] != 0; };
+  if (h.mask && std::all_of(h.mask, h.mask + B, [](unsigned char m) { return m == 0; })) return HMPC_OK;
   if (g_fail_next_solves > 0) {
     g_fail_next_solves--;
     g_err = "injected failure (hmpc_debug_fail_next_solves)";
     return HMPC_ERR_CUDA;
   }
   CK(cudaSetDevice(c->device));
+  const int* shifts = nullptr;  // warm start (device_call): per-robot shifts from the pinned copy of h.shift
+  if (h.warm && c->warm_start && h.shift) {
+    memcpy(c->h_shift, h.shift, (size_t)B * sizeof(int));
+    shifts = c->h_shift;
+  }
+  if (runs_in_place(c, h)) return solve_in_place(c, h, shifts);
+  const bool zc = B <= ZERO_COPY_MAX;                  // zero-copy staging, in one chunk
+  const int nch = zc ? 1 : (c->pool ? 2 : NCHUNK);     // else the copy pipeline (no chunk is empty: B > ZERO_COPY_MAX)
+  const cudaStream_t sts[NCHUNK] = {c->stream, c->xstream[0], c->xstream[1], c->xstream[2]};
+  Chunk ch[NCHUNK];
+  Trace tr;
+  tr.mark();
+  for (int k = 0; k < nch; k++) {
+    const int b0 = (int)((long long)B * k / nch), nb = (int)((long long)B * (k + 1) / nch) - b0;
+    const size_t li = (size_t)k * hmpc::host_lists_ints(c->max_batch);
+    int* ref = c->cfg.refine ? c->d_ref + (size_t)k * (1 + (size_t)c->max_batch) : nullptr;
+    ch[k] = Chunk{b0, nb, sts[k], {}, c->h_cls + li, c->d_lists + li, ref};
+    if (int rc = stage_chunk(c, h, zc, ch[k], shifts, tr)) return rc;
+  }
+  int rc = HMPC_OK;
+  for (int k = 0; k < nch; k++) {
+    if (int e = finish_chunk(c, h, zc, ch[k], tr)) return e;
+    if (check_converged(h, c->rows(c->h_out, ch[k].b0, ch[k].nb).status, ch[k].b0, ch[k].nb)) rc = HMPC_ERR_NOT_CONVERGED;
+  }
+  tr.end(B);
+  return rc;
+}
+}  // namespace
+
+HMPC_EXTERNC int hmpc_solve_batch(hmpc_ctx* c, const update_data_t* in, int B, double* wrench_out, int* status)
+{
+  return hmpc_solve_batch_ex(c, in, B, wrench_out, nullptr, status);
+}
+
+HMPC_EXTERNC int hmpc_solve_batch_ex(hmpc_ctx* c, const update_data_t* in, int B, double* wrench_out, double* tau_out,
+                                     int* status)
+{
+  return solve_batch_impl(c, HostCall(in, B, wrench_out, tau_out, status));
+}
+
+HMPC_EXTERNC int hmpc_solve_batch_warm(hmpc_ctx* c, const update_data_t* in, int B, double* wrench_out, double* tau_out,
+                                       int* status, const int* shift)
+{
+  if (!in) { g_err = "hmpc_solve_batch_warm: bad argument (null records)"; return HMPC_ERR_ARG; }
+  return solve_batch_impl(c, HostCall(in, B, wrench_out, tau_out, status).warm_start(shift));
+}
+
+HMPC_EXTERNC int hmpc_solve_batch_masked(hmpc_ctx* c, const update_data_t* in, int B, const unsigned char* mask, double* wrench_out,
+                                         double* tau_out, int* status, const int* shift)
+{
+  if (!in || !mask) { g_err = "hmpc_solve_batch_masked: bad argument (null records or mask)"; return HMPC_ERR_ARG; }
+  return solve_batch_impl(c, HostCall(in, B, wrench_out, tau_out, status).warm_start(shift, mask));
+}
+
+HMPC_EXTERNC int hmpc_solve_batch_states(hmpc_ctx* c, const hmpc_state_t* in, int B, double dtMPC, double* wrench_out,
+                                         double* tau_out, int* status)
+{
+  return solve_batch_impl(c, HostCall(in, B, dtMPC, wrench_out, tau_out, status));
+}
+
+HMPC_EXTERNC int hmpc_solve_batch_states_warm(hmpc_ctx* c, const hmpc_state_t* in, int B, double dtMPC, double* wrench_out,
+                                              double* tau_out, int* status, const int* shift)
+{
+  if (!in) { g_err = "hmpc_solve_batch_states_warm: bad argument (null states)"; return HMPC_ERR_ARG; }
+  return solve_batch_impl(c, HostCall(in, B, dtMPC, wrench_out, tau_out, status).warm_start(shift));
+}
+
+HMPC_EXTERNC int hmpc_solve_batch_states_masked(hmpc_ctx* c, const hmpc_state_t* in, int B, const unsigned char* mask,
+                                                double dtMPC, double* wrench_out, double* tau_out, int* status, const int* shift)
+{
+  if (!in || !mask) { g_err = "hmpc_solve_batch_states_masked: bad argument (null states or mask)"; return HMPC_ERR_ARG; }
+  return solve_batch_impl(c, HostCall(in, B, dtMPC, wrench_out, tau_out, status).warm_start(shift, mask));
+}
+
+HMPC_EXTERNC int hmpc_solve_batch_sharded(hmpc_ctx* c, const update_data_t* in_local, int B_local, double* wrench_local,
+                                          int* status_local, float* d_all)
+{
+  if (!c || !c->nccl) { g_err = "hmpc_solve_batch_sharded: call hmpc_shard_init first"; return HMPC_ERR_ARG; }
+  if (B_local < 1 || B_local > c->max_batch) { g_err = "hmpc_solve_batch_sharded: every rank needs 1 <= B_local <= capacity"; return HMPC_ERR_ARG; }
+  CK(cudaSetDevice(c->device));
+  const int par = (int)(c->shard_tick++ & 1u);
   const size_t nw = (size_t)12 * c->horizon;
-  // pipeline over chunks: the host packs chunk k+1 while the GPU copies/solves chunk k, and converts the
-  // results of chunk k while later chunks are still in flight
-  static const int nch_env = getenv("HMPC_CHUNKS") ? atoi(getenv("HMPC_CHUNKS")) : 0;
-  int nch = B >= 512 ? 2 : 1;  // with helper threads packing is short: two chunks overlap copy-back with compute
-  if (!c->pool) nch = B >= 512 ? NCHUNK : (B >= 128 ? 2 : 1);
-  if (nch_env >= 1 && nch_env <= NCHUNK) nch = nch_env;
-  static const bool trace = getenv("HMPC_TRACE") != nullptr;
-  // zero-copy mode: the kernels read the packed records from, and write the results to, pinned host memory
-  // directly (UVA-mapped), so a tick has no copy launches at all.  For large batches the two-chunk copy pipeline
-  // wins because packing overlaps the kernels there (crossover ~1.5k robots).  HMPC_ZEROCOPY=0/1 forces a mode.
-  static const int zc_env = getenv("HMPC_ZEROCOPY") ? atoi(getenv("HMPC_ZEROCOPY")) : -1;
-  const bool zc = zc_env >= 0 ? (zc_env != 0) : (B <= 1536);
-  if (zc && nch_env < 1) nch = 1;
-  // warm start (hmpc_solve_batch_warm): the context's working sets, per-robot shifts from the pinned copy of `shift`
-  int* ws = (warm && c->warm_start) ? c->d_ws : nullptr;
-  const int* hsh = nullptr;
-  if (ws && shift) {
-    memcpy(c->h_shift, shift, (size_t)B * sizeof(int));
-    hsh = c->h_shift;
+  HostCall h(in_local, B_local, wrench_local, nullptr, status_local);
+  const bool in_place = runs_in_place(c, h);
+  if (d_all) {
+    // this tick's float results go to shard_buf[par]; the gather that last read it (two ticks ago) must be done before
+    // they overwrite it — a stream-side wait, the host does not block
+    CK(cudaStreamWaitEvent(c->stream, c->gathered[par], 0));
+    if (in_place) h.shard_wrench = c->shard_buf[par], h.shard_solved = c->solved;  // the kernels store them
   }
-  // in-place mode: records (or states), wrenches and status all live in buffers the caller registered
-  // (hmpc_pin_host_buffer): the kernels gather the live bytes of every update_data_t over PCIe, or the preparation kernel
-  // reads the states there, and double results are stored where the caller wants them — the call is launches + one
-  // synchronize
-  const bool in_pinned = in ? c->pinned(in, (size_t)B * sizeof(update_data_t)) : c->pinned(sin, (size_t)B * sizeof(hmpc_state_t));
-  if (zc_env != 0 && !c->pins.empty() && in_pinned && c->pinned(wrench_out, (size_t)B * nw * sizeof(double)) &&
-      (!status || c->pinned(status, (size_t)B * sizeof(int)))) {
-    // the device-resident chain on the caller's records (states: prepared into the context's d_rec first): class 0
-    // classifies on the way, overflow escalates on the device
-    int* ds = status ? status : reinterpret_cast<int*>(c->h_out + (size_t)c->max_batch * nw * 4);
-    float* dt_ = tau_out ? reinterpret_cast<float*>(c->h_out + (size_t)c->max_batch * (nw * 4 + 4)) : nullptr;
-    if (mask) memcpy(c->h_mask, mask, (size_t)B);  // pinned: the selection kernel reads it mapped
-    hmpc::SolveIO io;
-    io.raw = in;
-    if (sin) io.states = sin, io.records = c->d_rec, io.dt_mpc = dtMPC;
-    io.batch = B;
-    io.wrench = c->shard_out;
-    io.wrench64 = wrench_out;
-    io.status = ds;
-    io.tau = dt_;
-    io.ws = ws;
-    io.warm = ws != nullptr;
-    io.shifts = hsh;
-    io.mask = mask ? c->h_mask : nullptr;
-    int rc = enqueue_solve(c, io, c->stream);
-    if (rc != HMPC_OK) return rc;
-    if (c->shard_out) {
+  const int rc = solve_batch_impl(c, h);
+  if (rc != HMPC_OK && rc != HMPC_ERR_NOT_CONVERGED) return rc;
+  if (d_all) {
+    if (!in_place) {
+      // the staged path: put the float results on the device for the gather
+      std::vector<float> tmp((size_t)B_local * nw);
+      for (size_t i = 0; i < tmp.size(); i++) tmp[i] = (float)wrench_local[i];
+      CK(cudaMemcpyAsync(c->shard_buf[par], tmp.data(), tmp.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+      CK(cudaStreamSynchronize(c->stream));
       CK(cudaEventRecord(c->solved, c->stream));
-      c->shard_used = true;
     }
-    CK(cudaStreamSynchronize(c->stream));
-    bool all_ok = true;
-    for (int i = 0; i < B; i++)
-      if (listed(i)) all_ok &= (HMPC_STATUS_CODE(ds[i]) == 0);
-    if (tau_out)
-      for (int i = 0; i < B; i++)
-        if (listed(i))
-          for (int j = 0; j < 10; j++) tau_out[(size_t)i * 10 + j] = (double)dt_[(size_t)i * 10 + j];
-    if (!all_ok) { g_err = "hmpc_solve_batch: at least one instance did not reach a KKT point (see status[])"; return HMPC_ERR_NOT_CONVERGED; }
-    return HMPC_OK;
+    // the path's ONE collective: every rank's slice of float wrenches to every device, beside the next tick
+    CK(cudaStreamWaitEvent(c->gstream, c->solved, 0));
+    if (nccl_fail(g_nccl.AllGather(c->shard_buf[par], d_all, (size_t)B_local * nw, /* ncclFloat32 */ 7, c->nccl, c->gstream), "ncclAllGather"))
+      return HMPC_ERR_CUDA;
+    CK(cudaEventRecord(c->gathered[par], c->gstream));
   }
-  double tr[4 * NCHUNK + 2];
-  int ntr = 0;
-  auto now = []() { timespec ts; clock_gettime(CLOCK_MONOTONIC, &ts); return ts.tv_sec * 1e6 + ts.tv_nsec * 1e-3; };
-  if (trace) tr[ntr++] = now();
-  int lo[NCHUNK + 1];
-  for (int k = 0; k <= nch; k++) lo[k] = (int)((long long)B * k / nch);
-  cudaStream_t sts[NCHUNK] = {c->stream, c->xstream[0], c->xstream[1], c->xstream[2]};
-  hmpc::SolveIO io[NCHUNK];  // each chunk's device views of records, results, working sets and shifts
-  int* hblk[NCHUNK];         // and its host-built lists
-  for (int k = 0; k < nch; k++) {
-    const int b0 = lo[k], nb = lo[k + 1] - lo[k];
-    if (nb == 0) continue;
-    int rc = HMPC_OK;
-    if (sin) {
-      // row f-1: ship the 352-byte states and build the packed records on the device (in a masked call the unlisted
-      // robots' records are built too, and not read)
-      const size_t sb = sizeof(hmpc_state_t);
-      memcpy(c->h_states + (size_t)b0 * sb, sin + b0, (size_t)nb * sb);
-      if (trace) tr[ntr++] = now();
-      if (!zc) CK(cudaMemcpyAsync(c->d_states + (size_t)b0 * sb, c->h_states + (size_t)b0 * sb, (size_t)nb * sb, cudaMemcpyHostToDevice, sts[k]));
-      rc = hmpc_prepare_device(c, reinterpret_cast<const hmpc_state_t*>((zc ? c->h_states : c->d_states) + (size_t)b0 * sb), nb, dtMPC,
-                               c->d_rec + (size_t)b0 * c->rec_stride, sts[k]);
-      if (rc != HMPC_OK) return rc;
-    } else {
-      // robots [r0, r1): all of them, or only the listed ones (the kernels read no other record)
-      auto pack = [&](int r0, int r1) {
-        if (!mask) return hmpc_pack_records(in + r0, r1 - r0, c->horizon, c->h_rec + (size_t)r0 * c->rec_stride);
-        for (int i = r0; i < r1; i++)
-          if (mask[i]) hmpc_pack_records(in + i, 1, c->horizon, c->h_rec + (size_t)i * c->rec_stride);
-        return (int)HMPC_OK;
-      };
-      if (c->pool && nb >= 128) {
-        c->pool->parallel([&](int part, int nparts) {
-          const int p0 = (int)((long long)nb * part / nparts), p1 = (int)((long long)nb * (part + 1) / nparts);
-          pack(b0 + p0, b0 + p1);
-        });
-      } else {
-        rc = pack(b0, b0 + nb);
-      }
-      if (rc != HMPC_OK) return rc;
-      if (trace) tr[ntr++] = now();
-      if (!zc)
-        CK(cudaMemcpyAsync(c->d_rec + (size_t)b0 * c->rec_stride, c->h_rec + (size_t)b0 * c->rec_stride,
-                           (size_t)nb * c->rec_stride, cudaMemcpyHostToDevice, sts[k]));
-    }
-    const size_t ooff = (size_t)b0 * (nw * 4 + 4 + 40), obytes = (size_t)nb * (nw * 4 + 4 + (tau_out ? 40 : 0));
-    unsigned char* obase = zc ? c->h_out : c->d_out;
-    io[k].records = ((zc && !sin) ? c->h_rec : c->d_rec) + (size_t)b0 * c->rec_stride;
-    io[k].batch = nb;
-    io[k].wrench = reinterpret_cast<float*>(obase + ooff);
-    io[k].status = reinterpret_cast<int*>(obase + ooff + (size_t)nb * nw * 4);
-    io[k].tau = tau_out ? reinterpret_cast<float*>(obase + ooff + (size_t)nb * (nw * 4 + 4)) : nullptr;
-    io[k].ws = ws ? ws + (size_t)b0 * hmpc::WS_STATE_INTS : nullptr;
-    io[k].warm = ws != nullptr;
-    if (hsh && zc) {
-      io[k].shifts = hsh + b0;  // mapped, like the records and lists of this mode
-    } else if (hsh) {
-      CK(cudaMemcpyAsync(c->d_shift + b0, hsh + b0, (size_t)nb * sizeof(int), cudaMemcpyHostToDevice, sts[k]));
-      io[k].shifts = c->d_shift + b0;
-    }
-    hblk[k] = c->h_cls + (size_t)k * hmpc::host_lists_ints(c->max_batch);
-    if (sin)
-      hmpc::classify_host(c->horizon, c->cfg.f_max, c->cls[0].nb_hi, sin[b0].gait, sizeof(hmpc_state_t), nb, hblk[k], c->max_batch,
-                          mask ? mask + b0 : nullptr);
-    else
-      hmpc::classify_host(c->horizon, c->cfg.f_max, c->cls[0].nb_hi, in[b0].gait, sizeof(update_data_t), nb, hblk[k], c->max_batch,
-                          mask ? mask + b0 : nullptr);
-    rc = enqueue_solve_hostlists(c, io[k], hblk[k], sts[k], k, zc);
-    if (rc != HMPC_OK) return rc;
-    if (!zc) CK(cudaMemcpyAsync(c->h_out + ooff, c->d_out + ooff, obytes, cudaMemcpyDeviceToHost, sts[k]));
-    if (trace) tr[ntr++] = now();
-  }
-  bool all_ok = true;
-  for (int k = 0; k < nch; k++) {
-    const int b0 = lo[k], nb = lo[k + 1] - lo[k];
-    if (nb == 0) continue;
-    CK(cudaStreamSynchronize(sts[k]));
-    if (trace) tr[ntr++] = now();
-    const size_t ooff = (size_t)b0 * (nw * 4 + 4 + 40);
-    {  // working-set overflow (rare, massively degenerate optima): the overflowed instances escalate (enqueue_overflow_retry)
-      const int* hs = reinterpret_cast<const int*>(c->h_out + ooff + (size_t)nb * nw * 4);
-      bool overflow = false, not_spd = false;
-      for (int i = 0; i < nb; i++) overflow |= listed(b0 + i) && (HMPC_STATUS_CODE(hs[i]) == hmpc::ST_WS_CAP);
-      for (int i = 0; i < nb; i++) not_spd |= listed(b0 + i) && (HMPC_STATUS_CODE(hs[i]) == hmpc::ST_NOT_SPD);
-      const bool refine = c->cfg.refine && not_spd;  // instances handed to the refinement class (on its device-side list)
-      if (overflow || refine) {
-        int rc = overflow ? enqueue_overflow_retry(c, io[k], hblk[k], hs, sts[k], k, mask ? mask + b0 : nullptr) : HMPC_OK;
-        if (rc == HMPC_OK && refine) rc = enqueue_refine_retry(c, io[k], sts[k], k);
-        if (rc != HMPC_OK) return rc;
-        if (!zc)
-          CK(cudaMemcpyAsync(c->h_out + ooff, c->d_out + ooff, (size_t)nb * (nw * 4 + 4 + (tau_out ? 40 : 0)),
-                             cudaMemcpyDeviceToHost, sts[k]));
-        CK(cudaStreamSynchronize(sts[k]));
-      }
-    }
-    const float* src = reinterpret_cast<const float*>(c->h_out + ooff);
-    const int* hst = reinterpret_cast<const int*>(c->h_out + ooff + (size_t)nb * nw * 4);
-    double* dst = wrench_out + (size_t)b0 * nw;
-    const float* ht = reinterpret_cast<const float*>(c->h_out + ooff + (size_t)nb * (nw * 4 + 4));
-    if (mask) {  // the listed rows only
-      for (int i = 0; i < nb; i++) {
-        if (!mask[b0 + i]) continue;
-        for (size_t e = 0; e < nw; e++) dst[(size_t)i * nw + e] = (double)src[(size_t)i * nw + e];
-        if (tau_out)
-          for (int j = 0; j < 10; j++) tau_out[(size_t)(b0 + i) * 10 + j] = (double)ht[(size_t)i * 10 + j];
-        if (status) status[b0 + i] = hst[i];
-        if (HMPC_STATUS_CODE(hst[i]) != 0) all_ok = false;
-      }
-      continue;
-    }
-    if (tau_out)
-      for (int i = 0; i < nb * 10; i++) tau_out[(size_t)b0 * 10 + i] = (double)ht[i];
-    const size_t tot = (size_t)nb * nw;
-    if (c->pool && nb >= 128) {
-      c->pool->parallel([&](int part, int nparts) {
-        const size_t i0 = tot * part / nparts, i1 = tot * (part + 1) / nparts;
-        for (size_t i = i0; i < i1; i++) dst[i] = (double)src[i];
-      });
-    } else {
-      for (size_t i = 0; i < tot; i++) dst[i] = (double)src[i];
-    }
-    for (int i = 0; i < nb; i++) {
-      if (status) status[b0 + i] = hst[i];
-      if (HMPC_STATUS_CODE(hst[i]) != 0) all_ok = false;
-    }
-  }
-  if (trace) {
-    tr[ntr++] = now();
-    fprintf(stderr, "[hmpc trace] B=%d us since entry:", B);
-    for (int i = 1; i < ntr; i++) fprintf(stderr, " %.0f", tr[i] - tr[0]);
-    fprintf(stderr, "  (per chunk: packed, enqueued; then per chunk: synced; end)\n");
-  }
-  if (!all_ok) { g_err = "hmpc_solve_batch: at least one instance did not reach a KKT point (see status[])"; return HMPC_ERR_NOT_CONVERGED; }
-  return HMPC_OK;
+  return rc;
 }
 
 // ---------------------------------------------------------------------------------------------------

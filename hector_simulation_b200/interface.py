@@ -12,7 +12,7 @@ import os
 
 import numpy as np
 
-from .scenarios import UPDATE_DTYPE
+from .scenarios import STATE_DTYPE, UPDATE_DTYPE
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libhector_mpc_b200.so")
@@ -298,30 +298,13 @@ class BatchedMPC:
         for a in arrays:
             _check(lib().hmpc_unpin_host_buffer(self._h, a.ctypes.data))
 
-    def solve_batch(self, records: np.ndarray, strict: bool = True, out=None):
-        """Host-buffer path: H2D + kernels + D2H inside.  -> (wrench [B,12N] f64, status [B] i32).
-        `out=(wrench, status)` reuses caller-owned result arrays (what a C caller in a control loop does)."""
-        if records.dtype != UPDATE_DTYPE or not records.flags.c_contiguous:
-            records = np.ascontiguousarray(records, dtype=UPDATE_DTYPE)
-        B = records.shape[0]
-        if out is not None:
-            wrench, status = out
-            assert wrench.dtype == np.float64 and wrench.shape == (B, 12 * self.horizon) and wrench.flags.c_contiguous
-            assert status.dtype == np.int32 and status.shape == (B,)
-        else:
-            wrench = np.zeros((B, 12 * self.horizon), dtype=np.float64)
-            status = np.zeros(B, dtype=np.int32)
-        _check(lib().hmpc_solve_batch(self._h, records.ctypes.data, B, wrench.ctypes.data, status.ctypes.data),
-               allow_not_converged=not strict)
-        return wrench, status
-
-    def solve_batch_warm(self, records: np.ndarray, shift=None, torques: bool = False, strict: bool = True, out=None):
-        """solve_batch warm-started from each robot's working set of its last warm call (hmpc_solve_batch_warm).
-        `shift` int32 [B]: steps robot i's horizon moved since then (None: all 1; 0: same horizon; < 0: no history).
-        -> (wrench, status), or (wrench, tau, status) with torques=True."""
-        if records.dtype != UPDATE_DTYPE or not records.flags.c_contiguous:
-            records = np.ascontiguousarray(records, dtype=UPDATE_DTYPE)
-        B = records.shape[0]
+    def _host_call(self, fn, x, dtype, strict, out, torques=False, mask=None, dt_mpc=None, warm=False, shift=None):
+        """One host-buffer call fn(ctx, x, B, [mask], [dt_mpc], wrench, [tau], status, [shift]): `mask` and `dt_mpc` are passed
+        when given, `shift` with warm=True, and `tau` unless torques is None.  -> (wrench, status), or (wrench, tau, status)
+        with torques=True."""
+        if x.dtype != dtype or not x.flags.c_contiguous:
+            x = np.ascontiguousarray(x, dtype=dtype)
+        B = x.shape[0]
         if out is not None:
             wrench, status = out
             assert wrench.dtype == np.float64 and wrench.shape == (B, 12 * self.horizon) and wrench.flags.c_contiguous
@@ -330,14 +313,35 @@ class BatchedMPC:
             wrench = np.zeros((B, 12 * self.horizon), dtype=np.float64)
             status = np.zeros(B, dtype=np.int32)
         tau = np.zeros((B, 10), dtype=np.float64) if torques else None
-        if shift is not None:
-            shift = np.ascontiguousarray(shift, dtype=np.int32)
-            assert shift.shape == (B,)
-        _check(lib().hmpc_solve_batch_warm(self._h, records.ctypes.data, B, wrench.ctypes.data,
-                                           tau.ctypes.data if torques else None, status.ctypes.data,
-                                           shift.ctypes.data if shift is not None else None),
-               allow_not_converged=not strict)
+        args = [self._h, x.ctypes.data, B]
+        if mask is not None:
+            mask = np.ascontiguousarray(np.asarray(mask) != 0).view(np.uint8)
+            assert mask.shape == (B,)
+            args.append(mask.ctypes.data)
+        if dt_mpc is not None:
+            args.append(dt_mpc)
+        args.append(wrench.ctypes.data)
+        if torques is not None:
+            args.append(tau.ctypes.data if torques else None)
+        args.append(status.ctypes.data)
+        if warm:
+            if shift is not None:
+                shift = np.ascontiguousarray(shift, dtype=np.int32)
+                assert shift.shape == (B,)
+            args.append(shift.ctypes.data if shift is not None else None)
+        _check(fn(*args), allow_not_converged=not strict)
         return (wrench, tau, status) if torques else (wrench, status)
+
+    def solve_batch(self, records: np.ndarray, strict: bool = True, out=None):
+        """Host-buffer path: H2D + kernels + D2H inside.  -> (wrench [B,12N] f64, status [B] i32).
+        `out=(wrench, status)` reuses caller-owned result arrays (what a C caller in a control loop does)."""
+        return self._host_call(lib().hmpc_solve_batch, records, UPDATE_DTYPE, strict, out, torques=None)
+
+    def solve_batch_warm(self, records: np.ndarray, shift=None, torques: bool = False, strict: bool = True, out=None):
+        """solve_batch warm-started from each robot's working set of its last warm call (hmpc_solve_batch_warm).
+        `shift` int32 [B]: steps robot i's horizon moved since then (None: all 1; 0: same horizon; < 0: no history).
+        -> (wrench, status), or (wrench, tau, status) with torques=True."""
+        return self._host_call(lib().hmpc_solve_batch_warm, records, UPDATE_DTYPE, strict, out, torques, warm=True, shift=shift)
 
     def solve_batch_masked(self, records: np.ndarray, mask, shift=None, torques: bool = False, strict: bool = True, out=None):
         """solve_batch_warm of the robots with mask[i] != 0 only (hmpc_solve_batch_masked): `mask` bool or uint8 [B], `shift`
@@ -345,86 +349,16 @@ class BatchedMPC:
         arrays are new and unlisted rows hold zeros (a status of 0 there means "not solved", not "optimal"); with
         `out=(wrench, status)` they keep what the caller's arrays held.  strict: raise when a listed robot did not converge.
         -> (wrench, status), or (wrench, tau, status) with torques=True."""
-        if records.dtype != UPDATE_DTYPE or not records.flags.c_contiguous:
-            records = np.ascontiguousarray(records, dtype=UPDATE_DTYPE)
-        B = records.shape[0]
-        mask = np.ascontiguousarray(np.asarray(mask) != 0).view(np.uint8)
-        assert mask.shape == (B,)
-        if out is not None:
-            wrench, status = out
-            assert wrench.dtype == np.float64 and wrench.shape == (B, 12 * self.horizon) and wrench.flags.c_contiguous
-            assert status.dtype == np.int32 and status.shape == (B,)
-        else:
-            wrench = np.zeros((B, 12 * self.horizon), dtype=np.float64)
-            status = np.zeros(B, dtype=np.int32)
-        tau = np.zeros((B, 10), dtype=np.float64) if torques else None
-        if shift is not None:
-            shift = np.ascontiguousarray(shift, dtype=np.int32)
-            assert shift.shape == (B,)
-        _check(lib().hmpc_solve_batch_masked(self._h, records.ctypes.data, B, mask.ctypes.data, wrench.ctypes.data,
-                                             tau.ctypes.data if torques else None, status.ctypes.data,
-                                             shift.ctypes.data if shift is not None else None),
-               allow_not_converged=not strict)
-        return (wrench, tau, status) if torques else (wrench, status)
+        return self._host_call(lib().hmpc_solve_batch_masked, records, UPDATE_DTYPE, strict, out, torques, mask, warm=True, shift=shift)
 
     def solve_batch_torques(self, records: np.ndarray, strict: bool = True):
         """Host path with the leg-controller epilogue: -> (wrench [B,12N], tau [B,10], status [B])."""
-        records = np.ascontiguousarray(records, dtype=UPDATE_DTYPE)
-        B = records.shape[0]
-        wrench = np.zeros((B, 12 * self.horizon), dtype=np.float64)
-        tau = np.zeros((B, 10), dtype=np.float64)
-        status = np.zeros(B, dtype=np.int32)
-        _check(lib().hmpc_solve_batch_ex(self._h, records.ctypes.data, B, wrench.ctypes.data, tau.ctypes.data, status.ctypes.data),
-               allow_not_converged=not strict)
-        return wrench, tau, status
+        return self._host_call(lib().hmpc_solve_batch_ex, records, UPDATE_DTYPE, strict, None, torques=True)
 
     def solve_batch_states(self, states: np.ndarray, strict: bool = True, torques: bool = False, out=None, dt_mpc: float = 0.04):
         """Row f-1: `hmpc_state_t` records in, data preparation on the device.  In place when the states, wrench and status
         arrays are pinned (pin()).  -> (wrench, [tau,] status)."""
-        from .scenarios import STATE_DTYPE
-
-        if states.dtype != STATE_DTYPE or not states.flags.c_contiguous:
-            states = np.ascontiguousarray(states, dtype=STATE_DTYPE)
-        B = states.shape[0]
-        if out is not None:
-            wrench, status = out
-            assert wrench.dtype == np.float64 and wrench.shape == (B, 12 * self.horizon) and wrench.flags.c_contiguous
-            assert status.dtype == np.int32 and status.shape == (B,)
-        else:
-            wrench = np.zeros((B, 12 * self.horizon), dtype=np.float64)
-            status = np.zeros(B, dtype=np.int32)
-        tau = np.zeros((B, 10), dtype=np.float64) if torques else None
-        _check(lib().hmpc_solve_batch_states(self._h, states.ctypes.data, B, dt_mpc, wrench.ctypes.data,
-                                             tau.ctypes.data if torques else None, status.ctypes.data),
-               allow_not_converged=not strict)
-        return (wrench, tau, status) if torques else (wrench, status)
-
-    def _states_call(self, fn, states, mask, shift, torques, strict, out, dt_mpc):
-        from .scenarios import STATE_DTYPE
-
-        if states.dtype != STATE_DTYPE or not states.flags.c_contiguous:
-            states = np.ascontiguousarray(states, dtype=STATE_DTYPE)
-        B = states.shape[0]
-        if out is not None:
-            wrench, status = out
-            assert wrench.dtype == np.float64 and wrench.shape == (B, 12 * self.horizon) and wrench.flags.c_contiguous
-            assert status.dtype == np.int32 and status.shape == (B,)
-        else:
-            wrench = np.zeros((B, 12 * self.horizon), dtype=np.float64)
-            status = np.zeros(B, dtype=np.int32)
-        tau = np.zeros((B, 10), dtype=np.float64) if torques else None
-        if shift is not None:
-            shift = np.ascontiguousarray(shift, dtype=np.int32)
-            assert shift.shape == (B,)
-        args = [self._h, states.ctypes.data, B]
-        if mask is not None:
-            mask = np.ascontiguousarray(np.asarray(mask) != 0).view(np.uint8)
-            assert mask.shape == (B,)
-            args.append(mask.ctypes.data)
-        _check(fn(*args, dt_mpc, wrench.ctypes.data, tau.ctypes.data if torques else None, status.ctypes.data,
-                  shift.ctypes.data if shift is not None else None),
-               allow_not_converged=not strict)
-        return (wrench, tau, status) if torques else (wrench, status)
+        return self._host_call(lib().hmpc_solve_batch_states, states, STATE_DTYPE, strict, out, torques, dt_mpc=dt_mpc)
 
     def solve_batch_states_warm(self, states: np.ndarray, shift=None, torques: bool = False, strict: bool = True, out=None,
                                 dt_mpc: float = 0.04):
@@ -432,7 +366,8 @@ class BatchedMPC:
         `shift` int32 [B]: steps robot i's horizon moved since then (None: all 1; 0: same horizon; < 0: no history).
         In place when the states, wrench and status arrays are pinned (pin()).  -> (wrench, status), or (wrench, tau, status)
         with torques=True."""
-        return self._states_call(lib().hmpc_solve_batch_states_warm, states, None, shift, torques, strict, out, dt_mpc)
+        return self._host_call(lib().hmpc_solve_batch_states_warm, states, STATE_DTYPE, strict, out, torques, dt_mpc=dt_mpc,
+                               warm=True, shift=shift)
 
     def solve_batch_states_masked(self, states: np.ndarray, mask, shift=None, torques: bool = False, strict: bool = True,
                                   out=None, dt_mpc: float = 0.04):
@@ -441,7 +376,8 @@ class BatchedMPC:
         out=None the arrays are new and unlisted rows hold zeros (a status of 0 there means "not solved", not "optimal");
         with `out=(wrench, status)` they keep what the caller's arrays held.  strict: raise when a listed robot did not
         converge.  -> (wrench, status), or (wrench, tau, status) with torques=True."""
-        return self._states_call(lib().hmpc_solve_batch_states_masked, states, mask, shift, torques, strict, out, dt_mpc)
+        return self._host_call(lib().hmpc_solve_batch_states_masked, states, STATE_DTYPE, strict, out, torques, mask,
+                               dt_mpc=dt_mpc, warm=True, shift=shift)
 
     def prepare_device(self, d_states, B: int, d_records, stream=None, dt_mpc: float = 0.04) -> None:
         """Row f-1 on device-resident data: torch uint8 [B,352] states -> packed records [B,stride].

@@ -438,7 +438,8 @@ def test_contexts_of_different_horizons_coexist(torch_cuda):
 
 def test_sharded_entry_points_single_rank(torch_cuda):
     """hmpc_shard_* with a one-rank group: the slice comes back on the caller's arrays like hmpc_solve_batch, and the
-    (here trivial) ncclAllGather delivers the float wrenches to the device buffer, tick after tick (double-buffered)."""
+    (here trivial) ncclAllGather delivers the float wrenches to the device buffer, tick after tick (double-buffered), from
+    registered arrays (in place) and from unregistered ones (staged)."""
     torch = torch_cuda
     from hector_simulation_b200 import sharding
 
@@ -456,6 +457,18 @@ def test_sharded_entry_points_single_rank(torch_cuda):
         g = sh.backend.gathered()
         assert np.array_equal(g, w_ref.astype(np.float32))
     sh.close()
+    # unregistered arrays: the staged path solves, and the float wrenches are copied to the device for the gather
+    mpc = interface.BatchedMPC(B, N)
+    mpc.shard_init(0, 1, interface.BatchedMPC.shard_unique_id())
+    d_all = torch.zeros((B, 12 * N), dtype=torch.float32, device="cuda")
+    for tick in range(3):
+        w, s = np.zeros((B, 12 * N)), np.zeros(B, np.int32)
+        d_all.zero_()
+        mpc.solve_batch_sharded(recs, (w, s), d_all)
+        mpc.shard_wait()
+        assert np.array_equal(s, s_ref) and np.array_equal(w, w_ref)
+        assert np.array_equal(d_all.cpu().numpy(), w_ref.astype(np.float32))
+    mpc.close()
 
 
 @pytest.mark.parametrize("N", [5, 10, 16])

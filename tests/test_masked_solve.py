@@ -319,15 +319,17 @@ def test_captured_masked_solve_replays_with_other_masks():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("mode", ["zero_copy", "copy_pipeline", "in_place"])
-def test_host_modes_equal_the_device_path(mode):
+@pytest.mark.parametrize("mode", ["zero_copy", "copy_pipeline", "copy_pipeline_4", "in_place"])
+def test_host_modes_equal_the_device_path(mode, monkeypatch):
     """hmpc_solve_batch_masked against hmpc_solve_device_masked on the same records and masks, two calls (shift NULL, then
     per-robot shifts): listed wrenches rounded to float, torques and status words are equal; unlisted rows of the caller's
-    arrays keep their sentinels.  The copy pipeline runs above 1536 robots in two chunks; the degenerate records make the
-    host path re-solve overflowed robots."""
+    arrays keep their sentinels.  The copy pipeline runs above 1536 robots, in two chunks with helper threads and in four
+    without (copy_pipeline_4: HMPC_HOST_THREADS=1); the degenerate records make the host path re-solve overflowed robots."""
     import torch
 
-    B = 1800 if mode == "copy_pipeline" else 300
+    if mode == "copy_pipeline_4":
+        monkeypatch.setenv("HMPC_HOST_THREADS", "1")   # read by hmpc_create
+    B = 1800 if mode.startswith("copy_pipeline") else 300
     recs, at = _mix(B, 51, ndeg=6)
     host, dev = interface.BatchedMPC(B, N), interface.BatchedMPC(B, N)
     d_rec = torch.from_numpy(interface.pack_records(recs, N)).cuda()
