@@ -160,8 +160,10 @@ struct hmpc_ctx {
   // multi-GPU (one process per GPU, batch sharded): NCCL communicator + double-buffered float results for the gather
   void* nccl = nullptr;            // ncclComm_t
   int shard_rank = 0, shard_world = 1;
-  float* shard_buf[2] = {nullptr, nullptr};   // [max_batch][12N] this rank's results of tick t / t+1
-  unsigned shard_tick = 0;
+  // [max_batch][12N] this rank's results of tick t / t+1.  Every sharded call leaves each robot's latest row in
+  // shard_buf[(shard_tick - 1) & 1] (zeros before its first solve), gathering or not.
+  float* shard_buf[2] = {nullptr, nullptr};
+  unsigned shard_tick = 0;         // sharded calls that completed their buffer
   cudaStream_t gstream = nullptr;  // the gather runs here, behind `solved`, beside the next tick
   cudaEvent_t solved = nullptr, gathered[2] = {nullptr, nullptr};
   int* d_ws = nullptr;             // [max_batch][WS_STATE_INTS] working sets of the previous tick (closed-loop warm start)
@@ -276,6 +278,15 @@ int launch_prepare(const hmpc::PrepareArgs& pa, cudaStream_t st, bool pdl)
 {
   CK(launch_chain(hmpc::hmpc_prepare_kernel, dim3(hmpc::prepare_grid(pa.batch)), dim3(hmpc::PREPARE_THREADS), 0, st, pdl,
                   pa.states, pa.batch, pa.N, pa.dtMPC, pa.records, pa.rec_stride, pa.list, pa.count));
+  CK(cudaGetLastError());
+  return HMPC_OK;
+}
+
+// the carry kernel (hmpc_chain.h: carry_grid): rows of `cur` the mask does not list get their bytes from `prev`
+int launch_carry(const unsigned char* mask, int batch, int N, const float* prev, float* cur, cudaStream_t st)
+{
+  hmpc::hmpc_carry_kernel<<<hmpc::carry_grid(batch, N), hmpc::CARRY_THREADS, 0, st>>>(
+      mask, batch, hmpc::carry_row_vecs(N), reinterpret_cast<const float4*>(prev), reinterpret_cast<float4*>(cur));
   CK(cudaGetLastError());
   return HMPC_OK;
 }
@@ -405,6 +416,8 @@ HMPC_EXTERNC int hmpc_shard_init(hmpc_ctx* c, int rank, int world, const void* i
   CK(cudaEventCreateWithFlags(&c->solved, cudaEventDisableTiming));
   for (int i = 0; i < 2; i++) {
     CK(cudaMalloc(&c->shard_buf[i], (size_t)c->max_batch * nw * sizeof(float)));
+    // a robot no sharded call has solved yet is gathered as zeros (the masked calls carry unlisted rows forward)
+    CK(cudaMemsetAsync(c->shard_buf[i], 0, (size_t)c->max_batch * nw * sizeof(float), c->stream));
     CK(cudaEventCreateWithFlags(&c->gathered[i], cudaEventDisableTiming));
   }
   return HMPC_OK;
@@ -927,7 +940,8 @@ struct HostCall {
   bool warm = false;                         // propose each robot's working set of its last warm call, moved shift[i] steps
   const int* shift = nullptr;                // (null: one step each)
   const unsigned char* mask = nullptr;       // [batch]: only robots with mask[i] != 0 are solved and have their rows written
-  float* shard_wrench = nullptr;             // hmpc_solve_batch_sharded in place: the kernels also store float wrenches here,
+  float* shard_wrench = nullptr;             // the sharded calls in place: the kernels also store float wrenches here,
+  const float* shard_prev = nullptr;         // (masked) the carry kernel fills the unlisted rows from this buffer,
   cudaEvent_t shard_solved = nullptr;        // and this event is recorded behind them
   bool listed(int i) const { return !mask || mask[i] != 0; }
 };
@@ -986,6 +1000,8 @@ int solve_in_place(hmpc_ctx* c, const HostCall& h, const int* shifts)
   io.raw = h.records, io.states = h.states, io.dt_mpc = h.dt_mpc;
   io.wrench64 = h.wrench, io.shifts = shifts, io.mask = h.mask ? c->h_mask : nullptr;
   if (int rc = enqueue_solve(c, io, c->stream)) return rc;
+  if (h.shard_prev)
+    if (int rc = launch_carry(c->h_mask, h.batch, c->horizon, h.shard_prev, h.shard_wrench, c->stream)) return rc;
   if (h.shard_solved) CK(cudaEventRecord(h.shard_solved, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   if (h.tau)
@@ -1172,40 +1188,77 @@ HMPC_EXTERNC int hmpc_solve_batch_states_masked(hmpc_ctx* c, const hmpc_state_t*
   return solve_batch_impl(c, HostCall(in, B, dtMPC, wrench_out, tau_out, status).warm_start(shift, mask));
 }
 
-HMPC_EXTERNC int hmpc_solve_batch_sharded(hmpc_ctx* c, const update_data_t* in_local, int B_local, double* wrench_local,
-                                          int* status_local, float* d_all)
+namespace {
+// The sharded calls: the host-buffer call `h` on this rank's slice, then this tick's float rows into shard_buf[par] and,
+// with d_all, the gather of that buffer.  The rows of the robots `h` lists (all without a mask) are this call's results;
+// the carry kernel copies the others from the previous tick's buffer, so every row is the robot's latest.
+int solve_sharded(hmpc_ctx* c, HostCall h, float* d_all, const char* who)
 {
-  if (!c || !c->nccl) { g_err = "hmpc_solve_batch_sharded: call hmpc_shard_init first"; return HMPC_ERR_ARG; }
-  if (B_local < 1 || B_local > c->max_batch) { g_err = "hmpc_solve_batch_sharded: every rank needs 1 <= B_local <= capacity"; return HMPC_ERR_ARG; }
+  if (!c || !c->nccl) { g_err = std::string(who) + ": call hmpc_shard_init first"; return HMPC_ERR_ARG; }
+  if (h.batch < 1 || h.batch > c->max_batch) { g_err = std::string(who) + ": every rank needs 1 <= B_local <= capacity"; return HMPC_ERR_ARG; }
   CK(cudaSetDevice(c->device));
-  const int par = (int)(c->shard_tick++ & 1u);
+  const int B = h.batch, par = (int)(c->shard_tick & 1u);
   const size_t nw = (size_t)12 * c->horizon;
-  HostCall h(in_local, B_local, wrench_local, nullptr, status_local);
-  const bool in_place = runs_in_place(c, h);
-  if (d_all) {
-    // this tick's float results go to shard_buf[par]; the gather that last read it (two ticks ago) must be done before
-    // they overwrite it — a stream-side wait, the host does not block
-    CK(cudaStreamWaitEvent(c->stream, c->gathered[par], 0));
-    if (in_place) h.shard_wrench = c->shard_buf[par], h.shard_solved = c->solved;  // the kernels store them
-  }
+  float* cur = c->shard_buf[par];
+  const float* prev = c->shard_buf[par ^ 1];
+  const bool none = h.mask && std::all_of(h.mask, h.mask + B, [](unsigned char m) { return m == 0; });  // nothing is solved
+  // the gather that last read `cur` (two ticks ago) must be done before this tick overwrites it — a stream-side wait, the
+  // host does not block
+  CK(cudaStreamWaitEvent(c->stream, c->gathered[par], 0));
+  if (runs_in_place(c, h) && !none)  // the kernels store the listed rows, the carry the others, both before `solved`
+    h.shard_wrench = cur, h.shard_prev = h.mask ? prev : nullptr, h.shard_solved = c->solved;
   const int rc = solve_batch_impl(c, h);
   if (rc != HMPC_OK && rc != HMPC_ERR_NOT_CONVERGED) return rc;
-  if (d_all) {
-    if (!in_place) {
-      // the staged path: put the float results on the device for the gather
-      std::vector<float> tmp((size_t)B_local * nw);
-      for (size_t i = 0; i < tmp.size(); i++) tmp[i] = (float)wrench_local[i];
-      CK(cudaMemcpyAsync(c->shard_buf[par], tmp.data(), tmp.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-      CK(cudaStreamSynchronize(c->stream));
-      CK(cudaEventRecord(c->solved, c->stream));
+  if (!h.shard_solved) {
+    // staged (or nothing solved): the listed rows' float results from the caller's array, then the carry
+    if (!none) {
+      std::vector<float> tmp((size_t)B * nw);
+      for (int i = 0; i < B; i++)
+        if (h.listed(i))
+          for (size_t e = 0; e < nw; e++) tmp[i * nw + e] = (float)h.wrench[i * nw + e];
+      CK(cudaMemcpyAsync(cur, tmp.data(), tmp.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
     }
+    if (h.mask) {
+      memcpy(c->h_mask, h.mask, (size_t)B);  // pinned: read mapped, like the selection kernel's
+      if (int e = launch_carry(c->h_mask, B, c->horizon, prev, cur, c->stream)) return e;
+    }
+    CK(cudaEventRecord(c->solved, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+  }
+  c->shard_tick++;
+  if (d_all) {
     // the path's ONE collective: every rank's slice of float wrenches to every device, beside the next tick
     CK(cudaStreamWaitEvent(c->gstream, c->solved, 0));
-    if (nccl_fail(g_nccl.AllGather(c->shard_buf[par], d_all, (size_t)B_local * nw, /* ncclFloat32 */ 7, c->nccl, c->gstream), "ncclAllGather"))
+    if (nccl_fail(g_nccl.AllGather(cur, d_all, (size_t)B * nw, /* ncclFloat32 */ 7, c->nccl, c->gstream), "ncclAllGather"))
       return HMPC_ERR_CUDA;
     CK(cudaEventRecord(c->gathered[par], c->gstream));
   }
   return rc;
+}
+}  // namespace
+
+HMPC_EXTERNC int hmpc_solve_batch_sharded(hmpc_ctx* c, const update_data_t* in_local, int B_local, double* wrench_local,
+                                          int* status_local, float* d_all)
+{
+  return solve_sharded(c, HostCall(in_local, B_local, wrench_local, nullptr, status_local), d_all, "hmpc_solve_batch_sharded");
+}
+
+HMPC_EXTERNC int hmpc_solve_batch_sharded_warm(hmpc_ctx* c, const update_data_t* in_local, int B_local,
+                                               const unsigned char* mask_local, double* wrench_local, double* tau_local,
+                                               int* status_local, const int* shift_local, float* d_all)
+{
+  if (!in_local) { g_err = "hmpc_solve_batch_sharded_warm: bad argument (null records)"; return HMPC_ERR_ARG; }
+  return solve_sharded(c, HostCall(in_local, B_local, wrench_local, tau_local, status_local).warm_start(shift_local, mask_local),
+                       d_all, "hmpc_solve_batch_sharded_warm");
+}
+
+HMPC_EXTERNC int hmpc_solve_batch_states_sharded_warm(hmpc_ctx* c, const hmpc_state_t* in_local, int B_local,
+                                                      const unsigned char* mask_local, double dtMPC, double* wrench_local,
+                                                      double* tau_local, int* status_local, const int* shift_local, float* d_all)
+{
+  if (!in_local) { g_err = "hmpc_solve_batch_states_sharded_warm: bad argument (null states)"; return HMPC_ERR_ARG; }
+  return solve_sharded(c, HostCall(in_local, B_local, dtMPC, wrench_local, tau_local, status_local).warm_start(shift_local, mask_local),
+                       d_all, "hmpc_solve_batch_states_sharded_warm");
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -260,6 +260,14 @@ inline PrepareArgs prepare_args(int N, const SolveIO& io, const ChainLists& list
   return pa;
 }
 
+// The carry launch of a sharded masked call (hmpc_carry_kernel), behind the chain: one thread per 16-byte vector of the
+// batch's float wrench rows, carry_grid(batch, N) CTAs of CARRY_THREADS.
+inline int carry_row_vecs(int N) { return 3 * N; }  // a row is 12N floats = 48N bytes
+inline int carry_grid(int batch, int N)
+{
+  return (int)(((long long)batch * carry_row_vecs(N) + CARRY_THREADS - 1) / CARRY_THREADS);
+}
+
 // The arguments of the launch of class `cls` (0-2, or REFINE_CLASS: the refinement class over lists.ref_list), shaped `k`.
 inline KernelArgs launch_args(const SolverSettings& S, int N, int ncls, int cls, const ClassCfg& k, const SolveIO& io,
                               const ChainLists& lists)

@@ -2409,4 +2409,20 @@ __global__ void __launch_bounds__(NT) hmpc_select_kernel(const unsigned char* ma
   if (tid == 0) *count = base;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Sharded masked calls (hmpc_solve_batch_sharded_warm): the gather sends every robot's latest float wrench row, but the
+// solve writes only the listed rows of this tick's buffer.  This kernel copies the unlisted rows from the previous tick's
+// buffer, one 16-byte vector per thread (a row of 12N floats is 3N vectors).  It writes no row the solve writes, so it
+// needs no ordering against the solve chain.  Launch shape: hmpc_chain.h, carry_grid.
+// ------------------------------------------------------------------------------------------------
+constexpr int CARRY_THREADS = 256;
+
+__global__ void __launch_bounds__(CARRY_THREADS) hmpc_carry_kernel(const unsigned char* mask, int batch, int row_vecs,
+                                                                    const float4* prev, float4* cur)
+{
+  const long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= (long long)batch * row_vecs) return;
+  if (mask[v / row_vecs] == 0) cur[v] = prev[v];
+}
+
 }  // namespace hmpc

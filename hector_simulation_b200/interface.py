@@ -33,6 +33,7 @@ EXPORTS = [
     "hmpc_set_refinement", "hmpc_reference_set_refinement",
     "hmpc_solve_device_masked", "hmpc_solve_batch_masked",
     "hmpc_solve_states_device_masked", "hmpc_solve_batch_states_warm", "hmpc_solve_batch_states_masked",
+    "hmpc_solve_batch_sharded_warm", "hmpc_solve_batch_states_sharded_warm",
 ]
 REFINEMENT_CLASS = 3  # hmpc_class_config index of the refinement class (HMPC_REFINEMENT_CLASS)
 
@@ -133,6 +134,11 @@ def lib() -> ctypes.CDLL:
         L.hmpc_solve_batch_states_masked.argtypes = ([ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_double]
                                                      + [ctypes.c_void_p] * 4)
         L.hmpc_solve_batch_states_masked.restype = ctypes.c_int
+        L.hmpc_solve_batch_sharded_warm.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 6
+        L.hmpc_solve_batch_sharded_warm.restype = ctypes.c_int
+        L.hmpc_solve_batch_states_sharded_warm.argtypes = ([ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_double]
+                                                           + [ctypes.c_void_p] * 5)
+        L.hmpc_solve_batch_states_sharded_warm.restype = ctypes.c_int
         _lib = L
     return _lib
 
@@ -298,10 +304,11 @@ class BatchedMPC:
         for a in arrays:
             _check(lib().hmpc_unpin_host_buffer(self._h, a.ctypes.data))
 
-    def _host_call(self, fn, x, dtype, strict, out, torques=False, mask=None, dt_mpc=None, warm=False, shift=None):
-        """One host-buffer call fn(ctx, x, B, [mask], [dt_mpc], wrench, [tau], status, [shift]): `mask` and `dt_mpc` are passed
-        when given, `shift` with warm=True, and `tau` unless torques is None.  -> (wrench, status), or (wrench, tau, status)
-        with torques=True."""
+    def _host_call(self, fn, x, dtype, strict, out, torques=False, mask=None, dt_mpc=None, warm=False, shift=None,
+                   sharded=False, d_all=None):
+        """One host-buffer call fn(ctx, x, B, [mask], [dt_mpc], wrench, [tau], status, [shift], [d_all]): `mask` and `dt_mpc`
+        are passed when given, `shift` with warm=True, `tau` unless torques is None, and with sharded=True the mask (or
+        NULL) and `d_all` (or NULL) always.  -> (wrench, status), or (wrench, tau, status) with torques=True."""
         if x.dtype != dtype or not x.flags.c_contiguous:
             x = np.ascontiguousarray(x, dtype=dtype)
         B = x.shape[0]
@@ -318,6 +325,8 @@ class BatchedMPC:
             mask = np.ascontiguousarray(np.asarray(mask) != 0).view(np.uint8)
             assert mask.shape == (B,)
             args.append(mask.ctypes.data)
+        elif sharded:
+            args.append(None)
         if dt_mpc is not None:
             args.append(dt_mpc)
         args.append(wrench.ctypes.data)
@@ -329,6 +338,8 @@ class BatchedMPC:
                 shift = np.ascontiguousarray(shift, dtype=np.int32)
                 assert shift.shape == (B,)
             args.append(shift.ctypes.data if shift is not None else None)
+        if sharded:
+            args.append(ctypes.c_void_p(d_all.data_ptr()) if d_all is not None else None)
         _check(fn(*args), allow_not_converged=not strict)
         return (wrench, tau, status) if torques else (wrench, status)
 
@@ -418,6 +429,19 @@ class BatchedMPC:
                                             ctypes.c_void_p(d_all.data_ptr()) if d_all is not None else None)
         _check(rc, allow_not_converged=not strict)
         return w, s
+
+    def solve_batch_sharded_warm(self, x: np.ndarray, out, d_all=None, mask=None, shift=None, torques: bool = False,
+                                 strict: bool = True, dt_mpc: float = 0.04):
+        """This rank's slice warm-started, optionally masked (hmpc_solve_batch_sharded_warm, or
+        hmpc_solve_batch_states_sharded_warm when `x` holds hmpc_state_t states): mask None is solve_batch_warm on the slice,
+        a mask is solve_batch_masked.  `out` = (wrench f64 [b,12N], status i32 [b]); `d_all` (torch CUDA f32 [world*b, 12N])
+        receives the all-gather, in which every robot's row is its latest result (zeros before its first solve).
+        -> (wrench, status), or (wrench, tau, status) with torques=True."""
+        if x.dtype == STATE_DTYPE:
+            return self._host_call(lib().hmpc_solve_batch_states_sharded_warm, x, STATE_DTYPE, strict, out, torques, mask,
+                                   dt_mpc=dt_mpc, warm=True, shift=shift, sharded=True, d_all=d_all)
+        return self._host_call(lib().hmpc_solve_batch_sharded_warm, x, UPDATE_DTYPE, strict, out, torques, mask, warm=True,
+                               shift=shift, sharded=True, d_all=d_all)
 
     def shard_wait(self) -> None:
         _check(lib().hmpc_shard_wait(self._h))

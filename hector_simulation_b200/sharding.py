@@ -6,6 +6,9 @@ the rank's own host arrays, in place) and the path's only exchange is ONE all-ga
 library (ncclAllGather on a side stream, overlapped with the next tick) when a consumer wants the whole batch on every
 device.  `ShardedMPC.tick` is the one function both bench.py (NCCL, GPUs) and tests/test_sharding_gloo.py (gloo, CPU, the
 oracle standing in for the local solve) drive; what differs is the `backend` that solves a slice and moves the gather.
+
+With warm=True a tick is hmpc_solve_batch_sharded_warm: warm-started, and with a mask only the due robots are solved; the
+gather still delivers every robot's latest wrench (zeros before its first solve).
 """
 from __future__ import annotations
 
@@ -37,8 +40,12 @@ class GpuBackend:
     def register(self, recs, out_w, out_s):
         self.mpc.pin(recs, out_w, out_s)      # the control loop's arrays: solved in place from now on
 
-    def solve(self, recs, out_w, out_s, gather: bool):
-        self.mpc.solve_batch_sharded(recs, (out_w, out_s), self.d_all if gather else None)
+    def solve(self, recs, out_w, out_s, gather: bool, warm: bool = False, mask=None, shift=None):
+        d_all = self.d_all if gather else None
+        if warm:
+            self.mpc.solve_batch_sharded_warm(recs, (out_w, out_s), d_all, mask=mask, shift=shift)
+        else:
+            self.mpc.solve_batch_sharded(recs, (out_w, out_s), d_all)
 
     def wait(self):
         self.mpc.shard_wait()
@@ -55,7 +62,9 @@ class GpuBackend:
 
 
 class TorchBackend:
-    """Any local solver + torch.distributed for the gather (the CPU test: oracle + gloo)."""
+    """Any local solver + torch.distributed for the gather (the CPU test: oracle + gloo).  The library's gather semantics:
+    solve_local sees the listed records only, and the gather sends every robot's latest row (zeros before its first
+    solve).  The solver stands in for a cold one, so `warm` and `shift` change nothing here."""
 
     def __init__(self, b_local: int, horizon: int, world: int, solve_local, group=None):
         import torch
@@ -64,17 +73,20 @@ class TorchBackend:
         self.torch, self.dist, self.group = torch, dist, group
         self.solve_local = solve_local
         self.all = torch.zeros((world * b_local, 12 * horizon), dtype=torch.float32)
+        self.latest = np.zeros((b_local, 12 * horizon), dtype=np.float32)
 
     def register(self, recs, out_w, out_s):
         pass
 
-    def solve(self, recs, out_w, out_s, gather: bool):
-        w, s = self.solve_local(recs)
-        out_w[:] = w
-        out_s[:] = s
+    def solve(self, recs, out_w, out_s, gather: bool, warm: bool = False, mask=None, shift=None):
+        rows = np.arange(len(recs)) if mask is None else np.flatnonzero(mask)
+        if len(rows):
+            w, s = self.solve_local(recs[rows])
+            out_w[rows] = w
+            out_s[rows] = s
+            self.latest[rows] = out_w[rows]
         if gather:
-            loc = self.torch.from_numpy(np.ascontiguousarray(out_w, dtype=np.float32))
-            self.dist.all_gather_into_tensor(self.all, loc, group=self.group)
+            self.dist.all_gather_into_tensor(self.all, self.torch.from_numpy(self.latest), group=self.group)
 
     def wait(self):
         pass
@@ -91,10 +103,14 @@ class ShardedMPC:
 
     tick(records_local) solves this rank's slice (padded to the common slice size with copies of its last record, so that
     every rank moves the same number of elements in the gather) and returns views of the slice's results;
-    whole_batch() assembles the gathered wrenches of the last tick in global robot order."""
+    whole_batch() assembles the gathered wrenches of the last tick in global robot order.  `record_dtype` is
+    scenarios.UPDATE_DTYPE (records) or scenarios.STATE_DTYPE (robot states, warm ticks only).
 
-    def __init__(self, batch: int, horizon: int, rank: int, world: int, backend_factory, record_dtype):
-        self.batch, self.horizon, self.rank, self.world = batch, horizon, rank, world
+    warm=True: every tick is warm-started, and tick(mask=..., shift=...) solves only the robots its mask lists; the padded
+    tail is never listed, so it is never solved."""
+
+    def __init__(self, batch: int, horizon: int, rank: int, world: int, backend_factory, record_dtype, warm: bool = False):
+        self.batch, self.horizon, self.rank, self.world, self.warm = batch, horizon, rank, world, warm
         self.bounds = shard_bounds(batch, world)
         self.lo, self.hi = self.bounds[rank]
         self.b_local = max(h - l for l, h in self.bounds)
@@ -105,6 +121,8 @@ class ShardedMPC:
         self.out_w = page_aligned((self.b_local, 12 * horizon), np.float64)
         self.out_s = page_aligned(self.b_local, np.int32)
         self.backend.register(self.recs, self.out_w, self.out_s)
+        self.mask = np.zeros(self.b_local, np.uint8)
+        self.shift = np.zeros(self.b_local, np.int32)
 
     def local_slice(self, records_global: np.ndarray) -> np.ndarray:
         return records_global[self.lo:self.hi]
@@ -115,7 +133,8 @@ class ShardedMPC:
         calls tick() without arguments — no copy, like hmpc_solve_batch on pinned arrays."""
         return self.recs
 
-    def tick(self, records_local: np.ndarray | None = None, gather: bool = True):
+    def tick(self, records_local: np.ndarray | None = None, gather: bool = True, mask=None, shift=None):
+        """mask / shift (warm ticks only): this rank's slices, [hi - lo] each; None lists every robot / moves each one step."""
         n = self.hi - self.lo
         if records_local is not None:
             assert len(records_local) == n
@@ -124,11 +143,26 @@ class ShardedMPC:
             self.recs[n:] = self.recs[n - 1]      # padding: a valid problem, its results are dropped
         elif n == 0:
             self.recs[:] = 0
-        self.backend.solve(self.recs, self.out_w, self.out_s, gather and self.world > 1)
+        if not self.warm:
+            assert mask is None and shift is None, "mask and shift need ShardedMPC(warm=True)"
+            self.backend.solve(self.recs, self.out_w, self.out_s, gather and self.world > 1)
+            return self.out_w[:n], self.out_s[:n]
+        m = None
+        if mask is not None or n < self.b_local:  # the padded tail is never listed
+            self.mask[:n] = 1 if mask is None else (np.asarray(mask) != 0)
+            self.mask[n:] = 0
+            m = self.mask
+        s = None
+        if shift is not None:
+            self.shift[:n] = shift
+            self.shift[n:] = 0
+            s = self.shift
+        self.backend.solve(self.recs, self.out_w, self.out_s, gather and self.world > 1, True, m, s)
         return self.out_w[:n], self.out_s[:n]
 
     def whole_batch(self) -> np.ndarray:
-        """[batch, 12N] float32 wrenches of the last tick(gather=True), global robot order."""
+        """[batch, 12N] float32 wrenches of the last tick(gather=True), global robot order: each robot's latest result (zeros
+        before its first solve)."""
         if self.world == 1:
             return self.out_w[: self.hi - self.lo].astype(np.float32)
         g = self.backend.gathered().reshape(self.world, self.b_local, 12 * self.horizon)

@@ -325,6 +325,28 @@ HMPC_EXTERNC int hmpc_shard_init(hmpc_ctx* ctx, int rank, int world, const void*
 HMPC_EXTERNC int hmpc_solve_batch_sharded(hmpc_ctx* ctx, const update_data_t* in_local, int B_local, double* wrench_local,
                                           int* status_local, float* d_all);
 HMPC_EXTERNC int hmpc_shard_wait(hmpc_ctx* ctx);
+/* Sharded calls warm-started, masked and on robot states: each rank solves only its due robots, and the gather still
+ * carries every robot's last wrench.
+ *   - mask_local NULL: hmpc_solve_batch_warm (hmpc_solve_batch_states_warm) on the local slice; non-NULL: the slice's
+ *     hmpc_solve_batch_masked (hmpc_solve_batch_states_masked).  The slice's results come back on the rank's own arrays in
+ *     all three host-buffer modes, in place when the arrays are pinned.  tau_local and shift_local may be NULL.
+ *   - Warm start: slot i is local robot i of this rank's context; shift_local as in the other warm calls.
+ *     hmpc_reset_warm_start and HMPC_WARM_START=0 act as elsewhere.
+ *   - HMPC_ERR_NOT_CONVERGED is returned for listed robots only.  Argument checks as in hmpc_solve_batch_sharded
+ *     (hmpc_shard_init first, 1 <= B_local <= capacity) plus those of the warm and masked calls.  An all-zero mask is
+ *     valid: nothing is solved, and the gather still runs.
+ *   - Gather: row r * B_local + i of d_all on every rank is the float wrench of robot i of rank r — this call's result
+ *     for a listed robot, else its row from the last sharded call of that context that solved it, or zeros if none has.
+ *     This holds whatever the caller's host arrays contain and whether or not earlier calls passed d_all: every sharded
+ *     call, hmpc_solve_batch_sharded included, keeps the context's gather buffers current, gathering or not.  A small
+ *     kernel behind the solve copies the unlisted rows from the previous tick's buffer. */
+HMPC_EXTERNC int hmpc_solve_batch_sharded_warm(hmpc_ctx* ctx, const struct update_data_t* in_local, int B_local,
+                                               const unsigned char* mask_local, double* wrench_local, double* tau_local,
+                                               int* status_local, const int* shift_local, float* d_all);
+HMPC_EXTERNC int hmpc_solve_batch_states_sharded_warm(hmpc_ctx* ctx, const struct hmpc_state_t* in_local, int B_local,
+                                                      const unsigned char* mask_local, double dtMPC, double* wrench_local,
+                                                      double* tau_local, int* status_local, const int* shift_local,
+                                                      float* d_all);
 
 /* Row f-4 (SURVEY.md §8f): the swing-leg controller, batched — swingLegController::updateSwingLeg
  * (src/common/SwingLegController.cpp:46-219): foot position, swing sub-phase (Gait::getSwingSubPhase,
