@@ -170,6 +170,8 @@ struct hmpc_ctx {
   int warm_start = 1;              // the warm calls propose them to the next tick (HMPC_WARM_START=0: cold start every tick)
   int* d_shift = nullptr;          // [max_batch] per-robot shifts of hmpc_solve_batch_warm (staged copy)
   int* h_shift = nullptr;          // pinned [max_batch] the same, also read mapped by the zero-copy and in-place modes
+  double* h_pred = nullptr;        // pinned [2][max_batch][12N]: wrenches in and plans out of a staged hmpc_predict_batch
+                                   // (allocated by the first one)
   // caller-owned host buffers registered with hmpc_pin_host_buffer: hmpc_solve_batch lets the kernels read the
   // reference records from them and write results to them in place (no packing, no staging copies, no widening)
   struct Pin { char* base; size_t bytes; };   // what the caller asked for
@@ -287,6 +289,17 @@ int launch_carry(const unsigned char* mask, int batch, int N, const float* prev,
 {
   hmpc::hmpc_carry_kernel<<<hmpc::carry_grid(batch, N), hmpc::CARRY_THREADS, 0, st>>>(
       mask, batch, hmpc::carry_row_vecs(N), reinterpret_cast<const float4*>(prev), reinterpret_cast<float4*>(cur));
+  CK(cudaGetLastError());
+  return HMPC_OK;
+}
+
+// the prediction kernel (hmpc_chain.h: predict_grid) over B rows of `rows`, row_stride bytes apart
+template <typename T>
+int launch_predict(const hmpc_ctx* c, const void* rows, int row_stride, int B, const unsigned char* mask, const T* wrench,
+                   T* pred, cudaStream_t st)
+{
+  hmpc::hmpc_predict_kernel<T><<<hmpc::predict_grid(B), hmpc::PREDICT_THREADS, 0, st>>>(
+      static_cast<const unsigned char*>(rows), row_stride, B, c->horizon, c->cfg.dt, mask, wrench, pred);
   CK(cudaGetLastError());
   return HMPC_OK;
 }
@@ -449,6 +462,7 @@ HMPC_EXTERNC void hmpc_destroy(hmpc_ctx* c)
   if (c->d_ws) cudaFree(c->d_ws);
   if (c->d_shift) cudaFree(c->d_shift);
   if (c->h_shift) cudaFreeHost(c->h_shift);
+  if (c->h_pred) cudaFreeHost(c->h_pred);
   if (c->h_mask) cudaFreeHost(c->h_mask);
   if (c->d_states) cudaFree(c->d_states);
   if (c->h_states) cudaFreeHost(c->h_states);
@@ -801,6 +815,69 @@ HMPC_EXTERNC int hmpc_solve_states_device_masked(hmpc_ctx* c, const hmpc_state_t
   io.states = d_states;
   io.dt_mpc = dtMPC;
   return enqueue_solve(c, io, static_cast<cudaStream_t>(stream));
+}
+
+// ---------------------------------------------------------------------------------------------------
+// the MPC's plan: predicted states under the discrete model of the solved QP (hmpc_predict_kernel)
+// ---------------------------------------------------------------------------------------------------
+HMPC_EXTERNC int hmpc_predict_device(hmpc_ctx* c, const void* d_records, int B, const unsigned char* d_mask, const float* d_wrench,
+                                     float* d_pred, void* stream)
+{
+  if (!c || !d_records || !d_wrench || !d_pred || B < 0 || B > c->max_batch) {
+    g_err = "hmpc_predict_device: bad argument (null pointer or batch > capacity)";
+    return HMPC_ERR_ARG;
+  }
+  if (B == 0) return HMPC_OK;
+  CK(cudaSetDevice(c->device));
+  return launch_predict(c, d_records, c->rec_stride, B, d_mask, d_wrench, d_pred, static_cast<cudaStream_t>(stream));
+}
+
+// test hook: 1 when the last hmpc_predict_batch that launched ran in place, 0 when it staged, -1 before any
+namespace { int g_predict_in_place = -1; }
+HMPC_EXTERNC int hmpc_debug_last_predict_in_place(void) { return g_predict_in_place; }
+
+// In place when the records, the wrenches and the plans lie in buffers registered with hmpc_pin_host_buffer: the kernel reads
+// the update_data_t rows and the double wrenches where they lie and writes the plans there.  Otherwise the listed robots'
+// first 19 floats go to the record staging (h_rec, record stride) and their wrenches to h_pred, which the kernel reads
+// mapped, and their plans come back from h_pred.  The same kernel on the same bytes: both modes give the same plans.
+HMPC_EXTERNC int hmpc_predict_batch(hmpc_ctx* c, const update_data_t* in, int B, const unsigned char* mask, const double* wrench,
+                                    double* pred_out)
+{
+  if (!c || !in || !wrench || !pred_out || B < 0 || B > c->max_batch) {
+    g_err = "hmpc_predict_batch: bad argument (null pointer or batch > capacity)";
+    return HMPC_ERR_ARG;
+  }
+  if (B == 0) return HMPC_OK;
+  if (mask && std::all_of(mask, mask + B, [](unsigned char m) { return m == 0; })) return HMPC_OK;
+  CK(cudaSetDevice(c->device));
+  const size_t nw = (size_t)12 * c->horizon, rs = (size_t)c->rec_stride;
+  const unsigned char* m = nullptr;
+  if (mask) {
+    memcpy(c->h_mask, mask, (size_t)B);  // pinned: the kernel reads it mapped
+    m = c->h_mask;
+  }
+  auto listed = [&](int i) { return !mask || mask[i] != 0; };
+  if (c->pinned(in, (size_t)B * sizeof(update_data_t)) && c->pinned(wrench, B * nw * sizeof(double)) &&
+      c->pinned(pred_out, B * nw * sizeof(double))) {
+    g_predict_in_place = 1;
+    if (int rc = launch_predict(c, in, (int)sizeof(update_data_t), B, m, wrench, pred_out, c->stream)) return rc;
+    CK(cudaStreamSynchronize(c->stream));
+    return HMPC_OK;
+  }
+  g_predict_in_place = 0;
+  if (!c->h_pred) CK(cudaMallocHost(&c->h_pred, 2 * (size_t)c->max_batch * nw * sizeof(double)));
+  double* hw = c->h_pred;
+  double* hp = c->h_pred + (size_t)c->max_batch * nw;
+  for (int i = 0; i < B; i++)
+    if (listed(i)) {
+      memcpy(c->h_rec + i * rs, in[i].p, 19 * sizeof(float));  // p v q w r, contiguous in update_data_t
+      memcpy(hw + i * nw, wrench + i * nw, nw * sizeof(double));
+    }
+  if (int rc = launch_predict(c, c->h_rec, c->rec_stride, B, m, hw, hp, c->stream)) return rc;
+  CK(cudaStreamSynchronize(c->stream));
+  for (int i = 0; i < B; i++)
+    if (listed(i)) memcpy(pred_out + i * nw, hp + i * nw, nw * sizeof(double));
+  return HMPC_OK;
 }
 
 HMPC_EXTERNC int hmpc_pin_host_buffer(hmpc_ctx* c, void* ptr, size_t bytes)

@@ -268,6 +268,14 @@ inline int carry_grid(int batch, int N)
   return (int)(((long long)batch * carry_row_vecs(N) + CARRY_THREADS - 1) / CARRY_THREADS);
 }
 
+// The prediction launch (hmpc_predict_kernel): one warp per robot, predict_grid(batch) CTAs of PREDICT_THREADS.  It is not
+// part of the chain: it runs behind the solve that wrote the wrenches, in plain stream order.
+inline int predict_grid(int batch)
+{
+  constexpr int warps = PREDICT_THREADS / 32;
+  return (batch + warps - 1) / warps;
+}
+
 // The arguments of the launch of class `cls` (0-2, or REFINE_CLASS: the refinement class over lists.ref_list), shaped `k`.
 inline KernelArgs launch_args(const SolverSettings& S, int N, int ncls, int cls, const ClassCfg& k, const SolveIO& io,
                               const ChainLists& lists)

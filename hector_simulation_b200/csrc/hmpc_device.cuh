@@ -2425,4 +2425,79 @@ __global__ void __launch_bounds__(CARRY_THREADS) hmpc_carry_kernel(const unsigne
   if (mask[v / row_vecs] == 0) cur[v] = prev[v];
 }
 
+// ------------------------------------------------------------------------------------------------
+// The MPC's plan (hmpc_predict_device, hmpc_predict_batch): robot i's predicted states x_{k+1} = Acd x_k + Bcd u_k,
+// k = 0..N-1, under the discrete model its QP was built from.  x_0, Acd and Bcd come from stage 1's own role_state and
+// role_inertia (float32, bit for bit the solve kernel's); u_k is wrench row entries [12k, 12k+12).  One warp per robot: the
+// roles run on the warp into its shared scratch, then lane r < 12 owns state component r through the N steps and reads the
+// others by shuffle.  The recurrence is float64 with separately rounded operations in a fixed order, row r:
+//   x_{k+1}[r] = x_k[r] + sum over the row's off-diagonal entries of Acd (ascending column, the gravity state last)
+//                       + sum over the row's entries of Bcd (ascending column)
+// where a row's entries are its structural ones: Acd is the identity plus dt*Rb (rows 0-2, columns 6-8), dt (rows 3-5,
+// columns 9-11) and -dt (row 11, column 12); Bcd fills rows 6-8 and two entries (i, i+3) of rows 9-11.  The gravity state
+// x[12] = 9.81f never changes and is not written.  Rows are read from `rows` with stride `row_stride`: only the first 19
+// floats (p v q w r), which lie at the same offsets in a packed record and in an update_data_t.  T is the element type of
+// the wrench in and the prediction out [B][N][12].  Robots with mask[i] == 0 (mask non-null) are skipped.  Launch shape:
+// hmpc_chain.h, predict_grid.
+// ------------------------------------------------------------------------------------------------
+constexpr int PREDICT_THREADS = 128;
+constexpr int PREDICT_WARP_BYTES = 1440;  // per warp: role scratch 64 B | x0 16 floats | Acd 169 | Bcd 156 floats
+
+template <typename T>
+__global__ void __launch_bounds__(PREDICT_THREADS) hmpc_predict_kernel(const unsigned char* rows, int row_stride, int batch,
+                                                                        int N, float dt, const unsigned char* mask,
+                                                                        const T* wrench, T* pred)
+{
+  constexpr int NW = PREDICT_THREADS / 32;
+  __shared__ __align__(16) unsigned char scratch[NW * PREDICT_WARP_BYTES];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int i = blockIdx.x * NW + wid;
+  if (i >= batch || (mask && mask[i] == 0)) return;  // (the whole warp)
+  unsigned char* scr = scratch + wid * PREDICT_WARP_BYTES;
+  float* x0f = reinterpret_cast<float*>(scr + 64);
+  float* Acd = x0f + 16;
+  float* Bcd = Acd + 169;  // (not zeroed: the roles write every entry read below)
+  const float* rf = reinterpret_cast<const float*>(rows + (size_t)i * row_stride);
+  role_state(rf, dt, x0f, Acd, lane, scr);
+  if (lane == 31) role_inertia(rf, dt, Bcd);
+  __syncwarp();
+  // lane r's row: nx entries of Acd on states xs[t], nu entries of Bcd on wrench entries us[t]
+  const int r = lane < 12 ? lane : 0;
+  const int nx = r < 3 ? 3 : (r < 6 || r == 11) ? 1 : 0;
+  const int nu = (r >= 6 && r < 9) ? 12 : (r >= 9 ? 2 : 0);
+  double ax[3], bu[12];
+  int xs[3], us[12];
+#pragma unroll
+  for (int t = 0; t < 3; t++) {
+    xs[t] = r < 3 ? 6 + t : (r < 6 ? r + 6 : 12);
+    ax[t] = t < nx ? (double)Acd[r * 13 + xs[t]] : 0.0;
+  }
+#pragma unroll
+  for (int t = 0; t < 12; t++) {
+    us[t] = r < 9 ? t : (t == 0 ? r - 9 : r - 6);
+    bu[t] = t < nu ? (double)Bcd[r * 12 + us[t]] : 0.0;
+  }
+  double x = lane < 13 ? (double)x0f[lane] : 0.0;
+  const T* w = wrench + (size_t)i * 12 * N;
+  T* out = pred + (size_t)i * 12 * N;
+  for (int k = 0; k < N; k++) {
+    const double u = lane < 12 ? (double)w[12 * k + lane] : 0.0;
+    double acc = x;
+#pragma unroll
+    for (int t = 0; t < 3; t++) {
+      const double v = __shfl_sync(0xffffffffu, x, xs[t]);
+      if (t < nx) acc = DA(acc, DM(ax[t], v));
+    }
+#pragma unroll
+    for (int t = 0; t < 12; t++) {
+      const double v = __shfl_sync(0xffffffffu, u, us[t]);
+      if (t < nu) acc = DA(acc, DM(bu[t], v));
+    }
+    if (lane < 12) {
+      x = acc;
+      out[12 * k + lane] = (T)acc;
+    }
+  }
+}
+
 }  // namespace hmpc

@@ -34,6 +34,7 @@ EXPORTS = [
     "hmpc_solve_device_masked", "hmpc_solve_batch_masked",
     "hmpc_solve_states_device_masked", "hmpc_solve_batch_states_warm", "hmpc_solve_batch_states_masked",
     "hmpc_solve_batch_sharded_warm", "hmpc_solve_batch_states_sharded_warm",
+    "hmpc_predict_device", "hmpc_predict_batch",
 ]
 REFINEMENT_CLASS = 3  # hmpc_class_config index of the refinement class (HMPC_REFINEMENT_CLASS)
 
@@ -139,6 +140,10 @@ def lib() -> ctypes.CDLL:
         L.hmpc_solve_batch_states_sharded_warm.argtypes = ([ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_double]
                                                            + [ctypes.c_void_p] * 5)
         L.hmpc_solve_batch_states_sharded_warm.restype = ctypes.c_int
+        L.hmpc_predict_device.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 4
+        L.hmpc_predict_device.restype = ctypes.c_int
+        L.hmpc_predict_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 3
+        L.hmpc_predict_batch.restype = ctypes.c_int
         _lib = L
     return _lib
 
@@ -292,7 +297,7 @@ class BatchedMPC:
 
     def pin(self, *arrays: np.ndarray) -> None:
         """Register caller-owned arrays (records or states, wrench, status) for the in-place mode of solve_batch and
-        solve_batch_states (and their _warm and _masked calls): the GPU then reads the records or states where they lie and writes the results where the caller wants them (hmpc_pin_host_buffer).
+        solve_batch_states (and their _warm and _masked calls), and of predict_batch: the GPU then reads the records or states where they lie and writes the results where the caller wants them (hmpc_pin_host_buffer).
         The arrays must stay alive until unpin()/close().  Registration pins whole pages: allocate the arrays with
         page_aligned() so that no unrelated heap object shares their pages (a later cudaMemcpy of such a neighbour, partly
         inside a registered page range, fails with cudaErrorInvalidValue)."""
@@ -510,6 +515,37 @@ class BatchedMPC:
                                                      d_records.data_ptr(), d_wrench.data_ptr(), d_status.data_ptr(),
                                                      d_tau.data_ptr() if d_tau is not None else None,
                                                      d_shift.data_ptr() if d_shift is not None else None, ctypes.c_void_p(st)))
+
+    def predict_device(self, d_records, B: int, d_wrench, d_pred, d_mask=None, stream=None) -> None:
+        """The MPC's plan on the device (hmpc_predict_device): robot i's predicted states under the discrete model its QP was
+        built from, d_pred[i, k] = x_{k+1} (rpy, p, omega, v: the layout of a record's traj).  torch CUDA tensors: records
+        uint8 [B,stride] (what the solve read), wrench f32 [B,12N] (what it wrote), d_pred f32 [B,N,12]; `d_mask` bool or
+        uint8 [B] or None (every robot): unlisted rows of d_pred keep their bytes.  A robot whose status code is not 0 has an
+        untrusted wrench, so its plan is untrusted too.  Enqueued on the current stream; capturable in a CUDA graph."""
+        import torch
+
+        st = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        _check(lib().hmpc_predict_device(self._h, d_records.data_ptr(), B, d_mask.data_ptr() if d_mask is not None else None,
+                                         d_wrench.data_ptr(), d_pred.data_ptr(), ctypes.c_void_p(st)))
+
+    def predict_batch(self, records: np.ndarray, wrench: np.ndarray, mask=None, out=None) -> np.ndarray:
+        """The MPC's plan from host buffers (hmpc_predict_batch): `records` update_data_t [B], `wrench` f64 [B,12N] as the
+        host solves return it -> f64 [B,N,12].  In place when records, wrench and `out` are pinned (pin()).  With a mask,
+        unlisted rows are not written: zeros in a new array, the caller's bytes in `out`."""
+        records = np.ascontiguousarray(records, dtype=UPDATE_DTYPE)
+        B, N = records.shape[0], self.horizon
+        wrench = np.ascontiguousarray(wrench, dtype=np.float64)
+        assert wrench.shape == (B, 12 * N)
+        if out is None:
+            out = np.zeros((B, N, 12), dtype=np.float64)
+        assert out.dtype == np.float64 and out.shape == (B, N, 12) and out.flags.c_contiguous
+        m = None
+        if mask is not None:
+            mask = np.ascontiguousarray(np.asarray(mask) != 0).view(np.uint8)
+            assert mask.shape == (B,)
+            m = mask.ctypes.data
+        _check(lib().hmpc_predict_batch(self._h, records.ctypes.data, B, m, wrench.ctypes.data, out.ctypes.data))
+        return out
 
     def assemble_device(self, d_records, B: int, stream=None) -> dict:
         """Parity hook: un-reduced fp32 QP data of B packed records (torch tensors on the GPU)."""

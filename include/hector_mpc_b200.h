@@ -298,6 +298,27 @@ HMPC_EXTERNC int hmpc_solve_batch_states_warm(hmpc_ctx* ctx, const struct hmpc_s
 HMPC_EXTERNC int hmpc_solve_batch_states_masked(hmpc_ctx* ctx, const struct hmpc_state_t* in, int B, const unsigned char* mask,
                                                 double dtMPC, double* wrench_out, double* tau_out, int* status,
                                                 const int* shift);
+/* The MPC's plan: robot i's predicted states under the discrete model its QP was built from, pred[i][k] = x_{k+1} =
+ * Acd x_k + Bcd u_k for k = 0 .. N-1, with x_0, Acd and Bcd the float32 ones of the solve (the same code computes them) and
+ * u_k = wrench row entries [12k, 12k+12).  A row of 12 is rpy, p, omega, v: the layout of update_data_t::traj, so pred - traj
+ * is the tracking error; the gravity state is not returned.  dt is the context's problem dt (hmpc_set_problem), as in the
+ * QP, not the caller's dtMPC.  The recurrence runs in float64 with separately rounded operations in a fixed order
+ * (DESIGN.md §3); hmpc_predict_device returns its float rounding.
+ *   - The plan is computed for whatever wrench row is passed.  A robot whose status code is not 0 has an untrusted wrench,
+ *     so its plan is untrusted too.
+ *   - A mask (NULL: every robot) skips robots with mask[i] == 0: their prediction rows keep their bytes.  Pass the mask of
+ *     the masked solve the wrenches came from.
+ *   - Argument checks: a NULL context or pointer and B > capacity are HMPC_ERR_ARG; B = 0 is a no-op.
+ *   hmpc_predict_device: d_records B packed records (or any rows whose first 19 floats are p v q w r) with row stride
+ *                        hmpc_record_bytes(horizon); d_wrench [B][12N] float; d_mask NULL or device bytes [B]; d_pred
+ *                        [B][N][12] float.  One launch on `stream`, no host synchronisation.  Capturable.
+ *   hmpc_predict_batch : in B update_data_t, wrench [B][12N] double as the host solves return them, mask NULL or host bytes
+ *                        [B], pred_out [B][N][12] double.  In place when in, wrench and pred_out lie in pinned ranges
+ *                        (hmpc_pin_host_buffer), else staged through the context's pinned memory; the same plans either way. */
+HMPC_EXTERNC int hmpc_predict_device(hmpc_ctx* ctx, const void* d_records, int B, const unsigned char* d_mask,
+                                     const float* d_wrench, float* d_pred, void* stream);
+HMPC_EXTERNC int hmpc_predict_batch(hmpc_ctx* ctx, const struct update_data_t* in, int B, const unsigned char* mask,
+                                    const double* wrench, double* pred_out);
 /* The reference boundary warm-started: after hmpc_reference_set_warm_start(1), every update_problem_data proposes the
  * previous call's working set moved one step (a hmpc_solve_batch_warm with shift NULL on the one-robot context).
  * setup_problem with another dt, f_max or horizon forgets it.  Default 0: every tick a cold start, like the reference. */
@@ -380,8 +401,8 @@ HMPC_EXTERNC int hmpc_swing_device(hmpc_ctx* ctx, const struct hmpc_state_t* d_s
 
 /* CUDA graphs.  The device-resident calls can be recorded into a CUDA graph by stream capture (cudaStreamBeginCapture,
  * torch.cuda.graph, ...) on the stream they are given: hmpc_solve_device, hmpc_solve_device_ex, hmpc_solve_device_warm,
- * hmpc_solve_device_masked, hmpc_solve_states_device_masked, hmpc_prepare_device, hmpc_rollout_device, hmpc_swing_device
- * and hmpc_reset_warm_start.  Each
+ * hmpc_solve_device_masked, hmpc_solve_states_device_masked, hmpc_prepare_device, hmpc_rollout_device, hmpc_swing_device,
+ * hmpc_predict_device and hmpc_reset_warm_start.  Each
  * launch of the graph gives the results an eager call on the same inputs gives, bit for bit.
  *   - A replay is a real call.  A captured warm solve proposes and records working sets, a captured rollout advances
  *     d_states and d_loop, a captured hmpc_reset_warm_start clears the working sets, every time the graph is launched.
@@ -393,7 +414,7 @@ HMPC_EXTERNC int hmpc_swing_device(hmpc_ctx* ctx, const struct hmpc_state_t* d_s
  *   - A call that returns an error while its stream is capturing may have recorded part of its work: end the capture
  *     and discard the graph.  Argument errors are found before anything is enqueued.
  * The host-buffer calls (hmpc_solve_batch, _ex, _warm, _masked, _states, _states_warm, _states_masked,
- * hmpc_solve_batch_sharded) and the reference boundary
+ * hmpc_solve_batch_sharded, hmpc_predict_batch) and the reference boundary
  * (update_problem_data) wait for their own streams and cannot be captured. */
 
 /* Robots beyond the conditioning limit (INTEGRATION.md).  The fp64 sweep inversion of the solve is accurate up to a scaled
