@@ -172,6 +172,8 @@ struct hmpc_ctx {
   int* h_shift = nullptr;          // pinned [max_batch] the same, also read mapped by the zero-copy and in-place modes
   double* h_pred = nullptr;        // pinned [2][max_batch][12N]: wrenches in and plans out of a staged hmpc_predict_batch
                                    // (allocated by the first one)
+  unsigned char* h_cert = nullptr; // pinned, max_batch x (row, wrench, certificate, multipliers) of a staged
+                                   // hmpc_certify_batch (allocated by the first one)
   // caller-owned host buffers registered with hmpc_pin_host_buffer: hmpc_solve_batch lets the kernels read the
   // reference records from them and write results to them in place (no packing, no staging copies, no widening)
   struct Pin { char* base; size_t bytes; };   // what the caller asked for
@@ -304,7 +306,30 @@ int launch_predict(const hmpc_ctx* c, const void* rows, int row_stride, int B, c
   return HMPC_OK;
 }
 
+// the certificate kernel (hmpc_chain.h: certify_grid) over B rows of `rows` in layout `lay`
+template <typename T>
+int launch_certify(const hmpc_ctx* c, const void* rows, hmpc::RowLayout lay, int B, const unsigned char* mask, const T* wrench,
+                   hmpc_certificate_t* cert, T* lambda, cudaStream_t st)
+{
+  hmpc::hmpc_certify_kernel<T><<<hmpc::certify_grid(B), hmpc::CERT_THREADS, 0, st>>>(
+      static_cast<const unsigned char*>(rows), lay, B, c->horizon, c->cfg.dt, c->cfg.f_max, mask, wrench,
+      reinterpret_cast<hmpc::CertOut*>(cert), lambda, nullptr);
+  CK(cudaGetLastError());
+  return HMPC_OK;
+}
+
 }  // namespace
+
+static_assert(sizeof(hmpc_certificate_t) == sizeof(hmpc::CertOut) && offsetof(hmpc_certificate_t, flags) ==
+              offsetof(hmpc::CertOut, flags), "hmpc_certificate_t is the kernel's CertOut");
+static_assert(HMPC_CERT_PASS == hmpc::CERT_PASS && HMPC_CERT_NONFINITE == hmpc::CERT_NONFINITE &&
+              HMPC_CERT_SWING == hmpc::CERT_SWING && HMPC_CERT_STATIONARITY == hmpc::CERT_STATIONARITY &&
+              HMPC_CERT_PRIMAL == hmpc::CERT_PRIMAL && HMPC_CERT_COMPLEMENTARITY == hmpc::CERT_COMPL,
+              "certificate flag bits");
+static_assert(HMPC_CERT_STATIONARITY_TOL == hmpc::CERT_STAT_TOL && HMPC_CERT_PRIMAL_TOL == hmpc::CERT_PRIMAL_TOL &&
+              HMPC_CERT_COMPLEMENTARITY_TOL == hmpc::CERT_COMPL_TOL, "certificate thresholds");
+static_assert(sizeof(update_data_t) == 3016 && offsetof(update_data_t, Alpha_K) == 1896 && offsetof(update_data_t, traj) == 168 &&
+              offsetof(update_data_t, gait) == 1944, "hmpc_chain.h: update_rows");
 
 // ---------------------------------------------------------------------------------------------------
 // records
@@ -463,6 +488,7 @@ HMPC_EXTERNC void hmpc_destroy(hmpc_ctx* c)
   if (c->d_shift) cudaFree(c->d_shift);
   if (c->h_shift) cudaFreeHost(c->h_shift);
   if (c->h_pred) cudaFreeHost(c->h_pred);
+  if (c->h_cert) cudaFreeHost(c->h_cert);
   if (c->h_mask) cudaFreeHost(c->h_mask);
   if (c->d_states) cudaFree(c->d_states);
   if (c->h_states) cudaFreeHost(c->h_states);
@@ -877,6 +903,76 @@ HMPC_EXTERNC int hmpc_predict_batch(hmpc_ctx* c, const update_data_t* in, int B,
   CK(cudaStreamSynchronize(c->stream));
   for (int i = 0; i < B; i++)
     if (listed(i)) memcpy(pred_out + i * nw, hp + i * nw, nw * sizeof(double));
+  return HMPC_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// the certificate: first-order optimality of a wrench for its row (hmpc_certify_kernel)
+// ---------------------------------------------------------------------------------------------------
+HMPC_EXTERNC int hmpc_certify_device(hmpc_ctx* c, const void* d_records, int B, const unsigned char* d_mask,
+                                     const float* d_wrench, hmpc_certificate_t* d_cert, float* d_lambda, void* stream)
+{
+  if (!c || !d_records || !d_wrench || !d_cert || B < 0 || B > c->max_batch) {
+    g_err = "hmpc_certify_device: bad argument (null pointer or batch > capacity)";
+    return HMPC_ERR_ARG;
+  }
+  if (B == 0) return HMPC_OK;
+  CK(cudaSetDevice(c->device));
+  return launch_certify(c, d_records, hmpc::packed_rows(c->horizon), B, d_mask, d_wrench, d_cert, d_lambda,
+                        static_cast<cudaStream_t>(stream));
+}
+
+// test hook: 1 when the last hmpc_certify_batch that launched ran in place, 0 when it staged, -1 before any
+namespace { int g_certify_in_place = -1; }
+HMPC_EXTERNC int hmpc_debug_last_certify_in_place(void) { return g_certify_in_place; }
+
+// In place when the rows, the wrenches, the certificates and the multipliers (when asked for) lie in registered buffers.
+// Otherwise the listed robots' update_data_t rows and wrenches go to h_cert, which the kernel reads mapped in the same
+// layout, and their certificates and multipliers come back from it.  The same kernel on the same bytes either way.
+HMPC_EXTERNC int hmpc_certify_batch(hmpc_ctx* c, const update_data_t* in, int B, const unsigned char* mask, const double* wrench,
+                                    hmpc_certificate_t* cert_out, double* lambda_out)
+{
+  if (!c || !in || !wrench || !cert_out || B < 0 || B > c->max_batch) {
+    g_err = "hmpc_certify_batch: bad argument (null pointer or batch > capacity)";
+    return HMPC_ERR_ARG;
+  }
+  if (B == 0) return HMPC_OK;
+  if (mask && std::all_of(mask, mask + B, [](unsigned char m) { return m == 0; })) return HMPC_OK;
+  CK(cudaSetDevice(c->device));
+  const size_t nw = (size_t)12 * c->horizon, nl = (size_t)16 * c->horizon;
+  const unsigned char* m = nullptr;
+  if (mask) {
+    memcpy(c->h_mask, mask, (size_t)B);  // pinned: the kernel reads it mapped
+    m = c->h_mask;
+  }
+  auto listed = [&](int i) { return !mask || mask[i] != 0; };
+  if (c->pinned(in, (size_t)B * sizeof(update_data_t)) && c->pinned(wrench, B * nw * sizeof(double)) &&
+      c->pinned(cert_out, B * sizeof(hmpc_certificate_t)) && (!lambda_out || c->pinned(lambda_out, B * nl * sizeof(double)))) {
+    g_certify_in_place = 1;
+    if (int rc = launch_certify(c, in, hmpc::update_rows(), B, m, wrench, cert_out, lambda_out, c->stream)) return rc;
+    CK(cudaStreamSynchronize(c->stream));
+    return HMPC_OK;
+  }
+  g_certify_in_place = 0;
+  const size_t mb = (size_t)c->max_batch;
+  if (!c->h_cert)
+    CK(cudaMallocHost(&c->h_cert, mb * (sizeof(update_data_t) + (nw + nl) * sizeof(double) + sizeof(hmpc_certificate_t))));
+  update_data_t* hr = reinterpret_cast<update_data_t*>(c->h_cert);
+  double* hw = reinterpret_cast<double*>(hr + mb);
+  double* hl = hw + mb * nw;
+  hmpc_certificate_t* hc = reinterpret_cast<hmpc_certificate_t*>(hl + mb * nl);
+  for (int i = 0; i < B; i++)
+    if (listed(i)) {
+      hr[i] = in[i];
+      memcpy(hw + i * nw, wrench + i * nw, nw * sizeof(double));
+    }
+  if (int rc = launch_certify(c, hr, hmpc::update_rows(), B, m, hw, hc, lambda_out ? hl : nullptr, c->stream)) return rc;
+  CK(cudaStreamSynchronize(c->stream));
+  for (int i = 0; i < B; i++)
+    if (listed(i)) {
+      cert_out[i] = hc[i];
+      if (lambda_out) memcpy(lambda_out + i * nl, hl + i * nl, nl * sizeof(double));
+    }
   return HMPC_OK;
 }
 

@@ -276,6 +276,18 @@ inline int predict_grid(int batch)
   return (batch + warps - 1) / warps;
 }
 
+// The certificate launch (hmpc_certify_kernel): one warp per robot, certify_grid(batch) CTAs of CERT_THREADS, behind the
+// wrenches it judges in plain stream order.  Its rows come in two layouts: the packed records of the device calls and the
+// update_data_t rows of the host calls.  The first 42 floats (state and weights) lie at the same offsets in both; Alpha_K,
+// traj and the gait bytes do not.
+inline int certify_grid(int batch)
+{
+  constexpr int warps = CERT_THREADS / 32;
+  return (batch + warps - 1) / warps;
+}
+inline RowLayout packed_rows(int N) { return RowLayout{record_stride(N), 42 * 4, 54 * 4, (54 + 12 * N) * 4}; }
+inline RowLayout update_rows() { return RowLayout{3016, 1896, 168, 1944}; }  // convexMPC_interface.h's update_data_t
+
 // The arguments of the launch of class `cls` (0-2, or REFINE_CLASS: the refinement class over lists.ref_list), shaped `k`.
 inline KernelArgs launch_args(const SolverSettings& S, int N, int ncls, int cls, const ClassCfg& k, const SolveIO& io,
                               const ChainLists& lists)

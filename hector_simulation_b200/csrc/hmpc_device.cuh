@@ -2440,6 +2440,49 @@ __global__ void __launch_bounds__(CARRY_THREADS) hmpc_carry_kernel(const unsigne
 // the wrench in and the prediction out [B][N][12].  Robots with mask[i] == 0 (mask non-null) are skipped.  Launch shape:
 // hmpc_chain.h, predict_grid.
 // ------------------------------------------------------------------------------------------------
+// One row of the plan's recurrence, x_{k+1}[r] = x_k[r] + (Acd x_k)[r] off the diagonal + (Bcd u_k)[r], on lane r < 12 of a
+// warp whose lane j holds x_k[j] (j < 13) and u_k[j] (j < 12): nx entries of Acd on states xs[t], nu entries of Bcd on
+// wrench entries us[t], in the order the comment of hmpc_predict_kernel gives.  ABS: the same sums over |Acd| and |Bcd|
+// (the caller passes |x| and |u|), the magnitude of the terms a state is formed from.  step() is called by the whole warp.
+template <bool ABS>
+struct PlanRow {
+  int nx, nu, xs[3], us[12];
+  double ax[3], bu[12];
+  __device__ __forceinline__ PlanRow(const float* Acd, const float* Bcd, int lane)
+  {
+    const int r = lane < 12 ? lane : 0;
+    nx = r < 3 ? 3 : (r < 6 || r == 11) ? 1 : 0;
+    nu = (r >= 6 && r < 9) ? 12 : (r >= 9 ? 2 : 0);
+#pragma unroll
+    for (int t = 0; t < 3; t++) {
+      xs[t] = r < 3 ? 6 + t : (r < 6 ? r + 6 : 12);
+      ax[t] = t < nx ? (double)Acd[r * 13 + xs[t]] : 0.0;
+      if (ABS) ax[t] = fabs(ax[t]);
+    }
+#pragma unroll
+    for (int t = 0; t < 12; t++) {
+      us[t] = r < 9 ? t : (t == 0 ? r - 9 : r - 6);
+      bu[t] = t < nu ? (double)Bcd[r * 12 + us[t]] : 0.0;
+      if (ABS) bu[t] = fabs(bu[t]);
+    }
+  }
+  __device__ __forceinline__ double step(double x, double u) const
+  {
+    double acc = x;
+#pragma unroll
+    for (int t = 0; t < 3; t++) {
+      const double v = __shfl_sync(0xffffffffu, x, xs[t]);
+      if (t < nx) acc = DA(acc, DM(ax[t], v));
+    }
+#pragma unroll
+    for (int t = 0; t < 12; t++) {
+      const double v = __shfl_sync(0xffffffffu, u, us[t]);
+      if (t < nu) acc = DA(acc, DM(bu[t], v));
+    }
+    return acc;
+  }
+};
+
 constexpr int PREDICT_THREADS = 128;
 constexpr int PREDICT_WARP_BYTES = 1440;  // per warp: role scratch 64 B | x0 16 floats | Acd 169 | Bcd 156 floats
 
@@ -2461,42 +2504,409 @@ __global__ void __launch_bounds__(PREDICT_THREADS) hmpc_predict_kernel(const uns
   role_state(rf, dt, x0f, Acd, lane, scr);
   if (lane == 31) role_inertia(rf, dt, Bcd);
   __syncwarp();
-  // lane r's row: nx entries of Acd on states xs[t], nu entries of Bcd on wrench entries us[t]
-  const int r = lane < 12 ? lane : 0;
-  const int nx = r < 3 ? 3 : (r < 6 || r == 11) ? 1 : 0;
-  const int nu = (r >= 6 && r < 9) ? 12 : (r >= 9 ? 2 : 0);
-  double ax[3], bu[12];
-  int xs[3], us[12];
-#pragma unroll
-  for (int t = 0; t < 3; t++) {
-    xs[t] = r < 3 ? 6 + t : (r < 6 ? r + 6 : 12);
-    ax[t] = t < nx ? (double)Acd[r * 13 + xs[t]] : 0.0;
-  }
-#pragma unroll
-  for (int t = 0; t < 12; t++) {
-    us[t] = r < 9 ? t : (t == 0 ? r - 9 : r - 6);
-    bu[t] = t < nu ? (double)Bcd[r * 12 + us[t]] : 0.0;
-  }
+  const PlanRow<false> row(Acd, Bcd, lane);
   double x = lane < 13 ? (double)x0f[lane] : 0.0;
   const T* w = wrench + (size_t)i * 12 * N;
   T* out = pred + (size_t)i * 12 * N;
   for (int k = 0; k < N; k++) {
     const double u = lane < 12 ? (double)w[12 * k + lane] : 0.0;
-    double acc = x;
-#pragma unroll
-    for (int t = 0; t < 3; t++) {
-      const double v = __shfl_sync(0xffffffffu, x, xs[t]);
-      if (t < nx) acc = DA(acc, DM(ax[t], v));
-    }
-#pragma unroll
-    for (int t = 0; t < 12; t++) {
-      const double v = __shfl_sync(0xffffffffu, u, us[t]);
-      if (t < nu) acc = DA(acc, DM(bu[t], v));
-    }
+    const double acc = row.step(x, u);
     if (lane < 12) {
       x = acc;
       out[12 * k + lane] = (T)acc;
     }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// The certificate (hmpc_certify_device, hmpc_certify_batch): a first-order optimality check of robot i's wrench U for its
+// row, independent of the solve.  One warp per robot, four per CTA (hmpc_chain.h: certify_grid).
+//   1. Roles: stage 1's role_leg, role_state and role_inertia into the warp's scratch: Fblk, x0, Acd and Bcd, the solve's
+//      float32 values bit for bit.
+//   2. Plan and cost: the recurrence of hmpc_predict_kernel (PlanRow), lane r < 12 owning state r, and beside it the same
+//      recurrence on |x0|, |Acd|, |Bcd|, |u|.  Lane r accumulates its cost terms in float64, step by step:
+//        c_r += (S_r e) e,  then  c_r += (alpha_r u) u,     e = x_{k+1}[r] - traj_k[r],  u = u_k[r]
+//      and J = c_0 + c_1 + ... + c_11 in that order: the QP objective 1/2 U'HU + g'U plus the constant d'Sd.
+//   3. Gradient: the adjoint sweep from k = N down to 1, p_{N+1} = 0, lane j:
+//        p_k[j] = p_{k+1}[j] + Acd[r][j] p_{k+1}[r] over column j's off-diagonal rows (ascending) + (2 S_j) e_k[j]
+//        grad u_{k-1}[c] = 0 + Bcd[r][c] p_k[r] over column c's rows (ascending) + (2 alpha_c) u_{k-1}[c]
+//      and the same sweep over the absolute values gives each entry the magnitude of its terms; the largest of them over
+//      the stance legs' entries is the robot's gradient scale.
+//   4. Multipliers: lane b < 2N owns block (step b/2, leg b%2).  A swing leg's six entries must be exactly 0.  A stance
+//      leg's 8 rows of Fblk, with stage 1's bounds (friction >= 0; 0 <= Mx <= 0.01; line contact <= 0; 0 <= Fz <= f_max
+//      gait; 5e10 means none), are candidates when their slack to a bound is within CERT_ACT_K eps P + CERT_ACT_ABS
+//      (eps: float32's, the precision of the rows; P: the robot's row scale below).  The block's gradient is fitted by the candidate rows with sign-constrained multipliers (>= 0 at a
+//      lower bound, <= 0 at an upper one) by Lawson-Hanson (cert_nnls), in float64 on the lane.
+//   5. Measures: stationarity = max |grad - A'lambda| / gradient scale; primal = the worst bound violation or non-zero
+//      swing entry / the largest sum |a||u| of the stance rows; complementarity = max |lambda| slack / (both scales).
+//      Thresholds CERT_*_TOL (DESIGN.md §7): the pass bit needs all three under them and finite inputs.
+// Rows are read through `lay` (hmpc_chain.h: packed_rows, update_rows).  T: wrench in and multipliers out (float: device
+// call, double: host call).  cert [B]; lambda NULL or [B][N][2][8] (signed, zero off the candidate rows and on swing
+// legs); grad NULL or [B][12N] (the gradient, for the kernel-source tests).  Robots with mask[i] == 0 are skipped.
+// ------------------------------------------------------------------------------------------------
+constexpr int CERT_THREADS = 128;
+constexpr int CERT_NMAX = 16;
+// per warp: role scratch 320 B | x0 16 floats | Acd 172 | Bcd 156 | Fblk 192 floats | plan, |plan|, gradient 3 x 192 doubles
+constexpr int CERT_WARP_BYTES = 320 + 4 * (16 + 172 + 156 + 192) + 3 * 8 * 12 * CERT_NMAX;
+// Candidate rows: slack <= CERT_ACT_K eps P + CERT_ACT_ABS, P the robot's row scale (the largest sum |a||u| of its stance
+// rows) and eps the float32 epsilon whatever T is: the rows and bounds are float32, so a row's value is defined to that
+// rounding whatever precision the wrench carries, and a solver holds its rows to its tolerance relative to the whole
+// problem, not to each foot's force: a foot at zero force comes back at ~1e-12 N (DESIGN.md §7).
+constexpr double CERT_EPS_ROWS = 1.1920928955078125e-07;
+constexpr double CERT_ACT_K = 64.0;
+constexpr double CERT_ACT_ABS = 1e-12;
+constexpr double CERT_NNLS_DUAL = 1e-14;   // a row enters when its dual exceeds this times max |grad| of the block
+constexpr int CERT_NNLS_ITERS = 64;        // Lawson-Hanson's outer iterations (a block has at most 6 independent rows)
+constexpr double CERT_NNLS_PIVOT = 1e-10;  // a row whose pivot falls below this times its norm^2 is dependent: left out
+constexpr double CERT_TINY = 1e-300;
+constexpr double CERT_STAT_TOL = 2e-6;     // (DESIGN.md §7: margins over the measured floors)
+constexpr double CERT_PRIMAL_TOL = 2e-7;
+constexpr double CERT_COMPL_TOL = 1e-9;
+enum : int { CERT_PASS = 1, CERT_NONFINITE = 2, CERT_SWING = 4, CERT_STATIONARITY = 8, CERT_PRIMAL = 16, CERT_COMPL = 32 };
+
+// where a row's Alpha_K, traj and gait bytes lie (byte offsets; the first 42 floats are common to both layouts)
+struct RowLayout {
+  int stride, alpha, traj, gait;
+};
+// one robot's certificate (include/hector_mpc_b200.h: hmpc_certificate_t)
+struct CertOut {
+  double cost, stationarity, primal, complementarity;
+  int n_active, flags;
+};
+
+__device__ __forceinline__ bool finite64(double x) { return fabs(x) <= 1.7976931348623157e308; }
+__device__ __forceinline__ double warp_max64(double v)
+{
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// min ||Z z - b|| over z restricted to the rows in bitmask P (Z: k rows of 6), by LDL' of the normal equations in a fixed
+// order; false when a pivot falls below CERT_NNLS_PIVOT times its diagonal (the rows in P are dependent)
+__device__ inline bool cert_ls(const double (*Z)[6], int k, unsigned P, const double* b, double* z)
+{
+  int p[8], np = 0;
+  for (int t = 0; t < k; t++)
+    if (P >> t & 1u) p[np++] = t;
+  double L[8][8], D[8], h[8];
+  for (int q = 0; q < np; q++) {
+    double hq = 0.0;
+    for (int c = 0; c < 6; c++) hq = DA(hq, DM(Z[p[q]][c], b[c]));
+    h[q] = hq;
+    for (int r = 0; r <= q; r++) {
+      double g = 0.0;
+      for (int c = 0; c < 6; c++) g = DA(g, DM(Z[p[q]][c], Z[p[r]][c]));
+      for (int t = 0; t < r; t++) g = DS(g, DM(DM(L[q][t], L[r][t]), D[t]));
+      if (r < q) {
+        L[q][r] = g / D[r];
+      } else {
+        double gqq = 0.0;
+        for (int c = 0; c < 6; c++) gqq = DA(gqq, DM(Z[p[q]][c], Z[p[q]][c]));
+        if (!(g > DM(CERT_NNLS_PIVOT, gqq))) return false;
+        D[q] = g;
+      }
+    }
+  }
+  for (int q = 0; q < np; q++) {
+    double v = h[q];
+    for (int t = 0; t < q; t++) v = DS(v, DM(L[q][t], h[t]));
+    h[q] = v;
+  }
+  for (int q = 0; q < np; q++) h[q] = h[q] / D[q];
+  for (int q = np - 1; q >= 0; q--) {
+    double v = h[q];
+    for (int t = q + 1; t < np; t++) v = DS(v, DM(L[t][q], h[t]));
+    h[q] = v;
+  }
+  for (int t = 0; t < k; t++) z[t] = 0.0;
+  for (int q = 0; q < np; q++) z[p[q]] = h[q];
+  return true;
+}
+
+// Lawson-Hanson: y >= 0 minimising ||Z'y - b|| over the k <= 8 rows of Z (one block's sign-flipped candidate rows)
+__device__ inline void cert_nnls(const double (*Z)[6], int k, const double* b, double* y)
+{
+  unsigned P = 0u, out = 0u;
+  double bmax = 0.0;
+  for (int c = 0; c < 6; c++) bmax = fmax(bmax, fabs(b[c]));
+  const double tol = DM(CERT_NNLS_DUAL, bmax);
+  for (int t = 0; t < 8; t++) y[t] = 0.0;
+  for (int it = 0; it < CERT_NNLS_ITERS; it++) {
+    double r[6];
+    for (int c = 0; c < 6; c++) {
+      double v = b[c];
+      for (int t = 0; t < k; t++)
+        if (P >> t & 1u) v = DS(v, DM(Z[t][c], y[t]));
+      r[c] = v;
+    }
+    int best = -1;
+    double wb = tol;
+    for (int t = 0; t < k; t++) {
+      if ((P | out) >> t & 1u) continue;
+      double w = 0.0;
+      for (int c = 0; c < 6; c++) w = DA(w, DM(Z[t][c], r[c]));
+      if (w > wb) {
+        wb = w;
+        best = t;
+      }
+    }
+    if (best < 0) break;
+    P |= 1u << best;
+    for (int inner = 0; inner < 8; inner++) {
+      double z[8];
+      // a row dependent on P, or one whose own multiplier comes out <= 0 (rounding), is left out until P changes
+      if (!cert_ls(Z, k, P, b, z) || (inner == 0 && !(z[best] > 0.0))) {
+        P &= ~(1u << best);
+        out |= 1u << best;
+        break;
+      }
+      out = 0u;
+      bool pos = true;
+      for (int t = 0; t < k; t++)
+        if ((P >> t & 1u) && !(z[t] > 0.0)) pos = false;
+      if (pos) {
+        for (int t = 0; t < k; t++) y[t] = (P >> t & 1u) ? z[t] : 0.0;
+        break;
+      }
+      double a = 2.0;
+      int tmin = -1;
+      for (int t = 0; t < k; t++)
+        if ((P >> t & 1u) && !(z[t] > 0.0)) {
+          const double at = y[t] / DS(y[t], z[t]);
+          if (at < a) {
+            a = at;
+            tmin = t;
+          }
+        }
+      if (tmin < 0) break;  // (non-finite z)
+      for (int t = 0; t < k; t++)
+        if (P >> t & 1u) y[t] = DA(y[t], DM(a, DS(z[t], y[t])));
+      y[tmin] = 0.0;
+      for (int t = 0; t < k; t++)
+        if ((P >> t & 1u) && !(y[t] > 0.0)) {
+          P &= ~(1u << t);
+          y[t] = 0.0;
+        }
+    }
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(CERT_THREADS) hmpc_certify_kernel(const unsigned char* rows, RowLayout lay, int batch, int N,
+                                                                     float dt, float f_max, const unsigned char* mask,
+                                                                     const T* wrench, CertOut* cert, T* lambda, double* grad)
+{
+  constexpr int NW = CERT_THREADS / 32;
+  __shared__ __align__(16) unsigned char scratch[NW * CERT_WARP_BYTES];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int i = blockIdx.x * NW + wid;
+  if (i >= batch || (mask && mask[i] == 0)) return;  // (the whole warp)
+  unsigned char* scr = scratch + wid * CERT_WARP_BYTES;
+  float* x0f = reinterpret_cast<float*>(scr + 320);
+  float* Acd = x0f + 16;
+  float* Bcd = Acd + 172;
+  float* Fblk = Bcd + 156;
+  double* X = reinterpret_cast<double*>(Fblk + 192);  // [N][12] x_{k+1}
+  double* XA = X + 12 * CERT_NMAX;                     // [N][12] the plan on absolute values
+  double* G = XA + 12 * CERT_NMAX;                     // [N][12] the gradient
+  const unsigned char* row = rows + (size_t)i * lay.stride;
+  const float* rf = reinterpret_cast<const float*>(row);
+  const float* alpha = reinterpret_cast<const float*>(row + lay.alpha);
+  const float* traj = reinterpret_cast<const float*>(row + lay.traj);
+  const unsigned char* gait = row + lay.gait;
+  const T* w = wrench + (size_t)i * 12 * N;
+
+  // ---- 1. the roles
+  for (int e = lane; e < 192; e += 32) Fblk[e] = 0.f;
+  __syncwarp();
+  role_leg(rf, lane, Fblk, scr);
+  __syncwarp();
+  role_state(rf, dt, x0f, Acd, lane, scr + 256);
+  if (lane == 31) role_inertia(rf, dt, Bcd);
+  __syncwarp();
+
+  // ---- 2. plan, its absolute-value twin and the cost
+  const int j = lane < 12 ? lane : 0;
+  const double S = (double)rf[30 + j], Al = (double)alpha[j];
+  bool fin = true;
+  double cost = 0.0;
+  {
+    const PlanRow<false> pr(Acd, Bcd, lane);
+    const PlanRow<true> pa(Acd, Bcd, lane);
+    double x = lane < 13 ? (double)x0f[lane] : 0.0, xa = fabs(x);
+    for (int k = 0; k < N; k++) {
+      const double u = lane < 12 ? (double)w[12 * k + lane] : 0.0;
+      const double nx = pr.step(x, u), na = pa.step(xa, fabs(u));
+      if (lane < 12) {
+        x = nx;
+        xa = na;
+        X[12 * k + lane] = x;
+        XA[12 * k + lane] = xa;
+        const double e = DS(x, (double)traj[12 * k + lane]);
+        cost = DA(cost, DM(DM(S, e), e));
+        cost = DA(cost, DM(DM(Al, u), u));
+        fin = fin && finite64(u) && finite64(x);
+      }
+    }
+  }
+  double J = 0.0;
+  for (int r = 0; r < 12; r++) J = DA(J, __shfl_sync(0xffffffffu, cost, r));
+  __syncwarp();
+
+  // ---- 3. the adjoint sweep and the gradient
+  double gscale = 0.0;
+  {
+    const int pn = (j >= 6 && j < 9) ? 3 : (j >= 9 ? 1 : 0);  // column j of Acd off the diagonal: rows ps[t]
+    const int bn = j < 6 ? 4 : 3;                               // column j of Bcd: rows bs[t]
+    int ps[3], bs[4];
+    double at[3], bt[4];
+#pragma unroll
+    for (int t = 0; t < 3; t++) {
+      ps[t] = j < 9 ? t : j - 6;
+      at[t] = t < pn ? (double)Acd[ps[t] * 13 + j] : 0.0;
+    }
+#pragma unroll
+    for (int t = 0; t < 4; t++) {
+      bs[t] = t < 3 ? 6 + t : 9 + j % 3;
+      bt[t] = t < bn ? (double)Bcd[bs[t] * 12 + j] : 0.0;
+    }
+    const double S2 = DM(2.0, S), A2 = DM(2.0, Al);
+    const int legj = leg_of(j);
+    double p = 0.0, q = 0.0;
+    for (int k = N; k >= 1; k--) {
+      double acc = p, acca = q;
+#pragma unroll
+      for (int t = 0; t < 3; t++) {
+        const double v = __shfl_sync(0xffffffffu, p, ps[t]), va = __shfl_sync(0xffffffffu, q, ps[t]);
+        if (t < pn) {
+          acc = DA(acc, DM(at[t], v));
+          acca = DA(acca, DM(fabs(at[t]), va));
+        }
+      }
+      const int o = 12 * (k - 1) + j;
+      const double xd = (double)traj[o];
+      p = DA(acc, DM(S2, DS(X[o], xd)));
+      q = DA(acca, DM(fabs(S2), DA(XA[o], fabs(xd))));
+      double g = 0.0, ga = 0.0;
+#pragma unroll
+      for (int t = 0; t < 4; t++) {
+        const double v = __shfl_sync(0xffffffffu, p, bs[t]), va = __shfl_sync(0xffffffffu, q, bs[t]);
+        if (t < bn) {
+          g = DA(g, DM(bt[t], v));
+          ga = DA(ga, DM(fabs(bt[t]), va));
+        }
+      }
+      const double u = (double)w[o];
+      g = DA(g, DM(A2, u));
+      ga = DA(ga, DM(fabs(A2), fabs(u)));
+      if (lane < 12) {
+        G[o] = g;
+        if (grad) grad[(size_t)i * 12 * N + o] = g;
+        const float fz = FM(f_max, (float)gait[2 * (k - 1) + legj]);
+        if (!(fz < 0.0001f && fz > -0.0001f)) gscale = fmax(gscale, ga);
+        fin = fin && finite64(g) && finite64(ga);
+      }
+    }
+  }
+  __syncwarp();
+
+  // ---- 4. one lane per (step, leg) block: rows, candidates, multipliers
+  double stat = 0.0, prim = 0.0, comp = 0.0, pscale = 0.0;
+  int nact = 0;
+  bool swing_bad = false;
+  const bool blk = lane < 2 * N;
+  const int s = lane >> 1, leg = lane & 1;
+  const float fz = blk ? FM(f_max, (float)gait[2 * s + leg]) : 0.f;
+  const bool stance = blk && !(fz < 0.0001f && fz > -0.0001f);
+  double u[6], v[8];
+  for (int c = 0; c < 6; c++) u[c] = blk ? (double)w[12 * s + col12_of(leg, c)] : 0.0;
+  if (stance) {
+    for (int t = 0; t < 8; t++) {
+      double vt = 0.0, rs = 0.0;
+      for (int c = 0; c < 6; c++) {
+        const double a = (double)Fblk[(8 * leg + t) * 12 + col12_of(leg, c)];
+        vt = DA(vt, DM(a, u[c]));
+        rs = DA(rs, DM(fabs(a), fabs(u[c])));
+      }
+      fin = fin && finite64(vt) && finite64(rs);
+      pscale = fmax(pscale, rs);
+      v[t] = vt;
+    }
+  }
+  pscale = warp_max64(pscale);
+  const double tol = DA(DM(DM(CERT_ACT_K, CERT_EPS_ROWS), pscale), CERT_ACT_ABS);
+  if (blk) {
+    T* lam = lambda ? lambda + (((size_t)i * N + s) * 2 + leg) * 8 : nullptr;
+    if (lam)
+      for (int t = 0; t < 8; t++) lam[t] = (T)0;
+    if (!stance) {
+      for (int c = 0; c < 6; c++)
+        if (u[c] != 0.0) {
+          swing_bad = true;
+          prim = fmax(prim, fabs(u[c]));
+        }
+    } else {
+      double Z[8][6], y[8], sl[8], gb[6];
+      int rowof[8], k = 0;
+      bool up[8];
+      for (int c = 0; c < 6; c++) gb[c] = G[12 * s + col12_of(leg, c)];
+      for (int t = 0; t < 8; t++) {
+        const bool haslo = t < 5 || t == 7, hashi = t >= 4;
+        const double hi = t == 4 ? (double)0.01f : (t == 7 ? (double)fz : 0.0);
+        const double slo = haslo ? v[t] : 1e300, shi = hashi ? DS(hi, v[t]) : 1e300;  // (lower bounds are 0)
+        prim = fmax(prim, fmax(-slo, -shi));
+        const bool atlo = slo <= tol, athi = shi <= tol;
+        if (atlo || athi) {
+          const bool upper = athi && (!atlo || shi < slo);
+          for (int c = 0; c < 6; c++) {
+            const double a = (double)Fblk[(8 * leg + t) * 12 + col12_of(leg, c)];
+            Z[k][c] = upper ? -a : a;
+          }
+          sl[k] = fabs(upper ? shi : slo);
+          up[k] = upper;
+          rowof[k++] = t;
+        }
+      }
+      cert_nnls(Z, k, gb, y);
+      nact = k;
+      double res[6];
+      for (int c = 0; c < 6; c++) res[c] = gb[c];
+      for (int t = 0; t < k; t++)
+        for (int c = 0; c < 6; c++) res[c] = DS(res[c], DM(y[t], Z[t][c]));
+      for (int c = 0; c < 6; c++) stat = fmax(stat, fabs(res[c]));
+      for (int t = 0; t < k; t++) {
+        comp = fmax(comp, DM(y[t], sl[t]));
+        if (lam) lam[rowof[t]] = (T)(up[t] ? -y[t] : y[t]);
+      }
+    }
+  }
+
+  // ---- 5. the robot's measures
+  gscale = warp_max64(gscale);
+  stat = warp_max64(stat);
+  prim = warp_max64(prim);
+  comp = warp_max64(comp);
+  for (int o = 16; o > 0; o >>= 1) nact += __shfl_xor_sync(0xffffffffu, nact, o);
+  const bool any_swing = __any_sync(0xffffffffu, swing_bad);
+  const bool all_fin = !__any_sync(0xffffffffu, !fin) && finite64(J);
+  if (lane == 0) {
+    CertOut c;
+    const double gs = fmax(gscale, CERT_TINY), pss = fmax(pscale, CERT_TINY);
+    c.cost = J;
+    c.stationarity = stat / gs;
+    c.primal = prim / pss;
+    c.complementarity = comp / DM(gs, pss);
+    c.n_active = nact;
+    int f = 0;
+    if (!all_fin) f |= CERT_NONFINITE;
+    if (any_swing) f |= CERT_SWING;
+    if (!(c.stationarity <= CERT_STAT_TOL)) f |= CERT_STATIONARITY;
+    if (!(c.primal <= CERT_PRIMAL_TOL)) f |= CERT_PRIMAL;
+    if (!(c.complementarity <= CERT_COMPL_TOL)) f |= CERT_COMPL;
+    if (f == 0) f = CERT_PASS;
+    c.flags = f;
+    cert[i] = c;
   }
 }
 

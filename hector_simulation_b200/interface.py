@@ -34,8 +34,12 @@ EXPORTS = [
     "hmpc_solve_device_masked", "hmpc_solve_batch_masked",
     "hmpc_solve_states_device_masked", "hmpc_solve_batch_states_warm", "hmpc_solve_batch_states_masked",
     "hmpc_solve_batch_sharded_warm", "hmpc_solve_batch_states_sharded_warm",
-    "hmpc_predict_device", "hmpc_predict_batch",
+    "hmpc_predict_device", "hmpc_predict_batch", "hmpc_certify_device", "hmpc_certify_batch",
 ]
+# hmpc_certificate_t, and its flag bits (include/hector_mpc_b200.h)
+CERTIFICATE_DTYPE = np.dtype([("cost", "<f8"), ("stationarity", "<f8"), ("primal", "<f8"), ("complementarity", "<f8"),
+                              ("n_active", "<i4"), ("flags", "<i4")])
+CERT_PASS, CERT_NONFINITE, CERT_SWING, CERT_STATIONARITY, CERT_PRIMAL, CERT_COMPLEMENTARITY = 1, 2, 4, 8, 16, 32
 REFINEMENT_CLASS = 3  # hmpc_class_config index of the refinement class (HMPC_REFINEMENT_CLASS)
 
 SETUP_DTYPE = np.dtype([("dt", "<f4"), ("mu", "<f4"), ("f_max", "<f4"), ("horizon", "<i4")], align=True)
@@ -144,6 +148,10 @@ def lib() -> ctypes.CDLL:
         L.hmpc_predict_device.restype = ctypes.c_int
         L.hmpc_predict_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 3
         L.hmpc_predict_batch.restype = ctypes.c_int
+        L.hmpc_certify_device.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 5
+        L.hmpc_certify_device.restype = ctypes.c_int
+        L.hmpc_certify_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 4
+        L.hmpc_certify_batch.restype = ctypes.c_int
         _lib = L
     return _lib
 
@@ -297,7 +305,7 @@ class BatchedMPC:
 
     def pin(self, *arrays: np.ndarray) -> None:
         """Register caller-owned arrays (records or states, wrench, status) for the in-place mode of solve_batch and
-        solve_batch_states (and their _warm and _masked calls), and of predict_batch: the GPU then reads the records or states where they lie and writes the results where the caller wants them (hmpc_pin_host_buffer).
+        solve_batch_states (and their _warm and _masked calls), and of predict_batch and certify_batch: the GPU then reads the records or states where they lie and writes the results where the caller wants them (hmpc_pin_host_buffer).
         The arrays must stay alive until unpin()/close().  Registration pins whole pages: allocate the arrays with
         page_aligned() so that no unrelated heap object shares their pages (a later cudaMemcpy of such a neighbour, partly
         inside a registered page range, fails with cudaErrorInvalidValue)."""
@@ -546,6 +554,44 @@ class BatchedMPC:
             m = mask.ctypes.data
         _check(lib().hmpc_predict_batch(self._h, records.ctypes.data, B, m, wrench.ctypes.data, out.ctypes.data))
         return out
+
+    def certify_device(self, d_records, B: int, d_wrench, d_cert, d_lambda=None, d_mask=None, stream=None) -> None:
+        """The certificate on the device (hmpc_certify_device): is robot i's wrench a KKT point of its record's QP?  torch
+        CUDA tensors: records uint8 [B,stride], wrench f32 [B,12N], d_cert uint8 [B,40] (view as CERTIFICATE_DTYPE on the
+        host), d_lambda f32 [B,N,2,8] or None; `d_mask` bool or uint8 [B] or None (every robot): unlisted rows keep their
+        bytes.  Enqueued on the current stream; capturable in a CUDA graph."""
+        import torch
+
+        st = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        _check(lib().hmpc_certify_device(self._h, d_records.data_ptr(), B, d_mask.data_ptr() if d_mask is not None else None,
+                                         d_wrench.data_ptr(), d_cert.data_ptr(),
+                                         d_lambda.data_ptr() if d_lambda is not None else None, ctypes.c_void_p(st)))
+
+    def certify_batch(self, records: np.ndarray, wrench: np.ndarray, mask=None, out=None, lam=None):
+        """The certificate from host buffers (hmpc_certify_batch): `records` update_data_t [B], `wrench` f64 [B,12N] ->
+        CERTIFICATE_DTYPE [B] (`out`), and with `lam` (f64 [B,N,2,8], or True for a new array) the multipliers:
+        -> (cert, lam).  In place when records, wrench, out and lam are pinned (pin()).  With a mask, unlisted rows are not
+        written."""
+        records = np.ascontiguousarray(records, dtype=UPDATE_DTYPE)
+        B, N = records.shape[0], self.horizon
+        wrench = np.ascontiguousarray(wrench, dtype=np.float64)
+        assert wrench.shape == (B, 12 * N)
+        if out is None:
+            out = np.zeros(B, CERTIFICATE_DTYPE)
+        assert out.dtype == CERTIFICATE_DTYPE and out.shape == (B,) and out.flags.c_contiguous
+        want_lam = lam is not None and lam is not False
+        if lam is True:
+            lam = np.zeros((B, N, 2, 8), np.float64)
+        if want_lam:
+            assert lam.dtype == np.float64 and lam.shape == (B, N, 2, 8) and lam.flags.c_contiguous
+        m = None
+        if mask is not None:
+            mask = np.ascontiguousarray(np.asarray(mask) != 0).view(np.uint8)
+            assert mask.shape == (B,)
+            m = mask.ctypes.data
+        _check(lib().hmpc_certify_batch(self._h, records.ctypes.data, B, m, wrench.ctypes.data, out.ctypes.data,
+                                        lam.ctypes.data if want_lam else None))
+        return (out, lam) if want_lam else out
 
     def assemble_device(self, d_records, B: int, stream=None) -> dict:
         """Parity hook: un-reduced fp32 QP data of B packed records (torch tensors on the GPU)."""

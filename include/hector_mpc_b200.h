@@ -319,6 +319,48 @@ HMPC_EXTERNC int hmpc_predict_device(hmpc_ctx* ctx, const void* d_records, int B
                                      const float* d_wrench, float* d_pred, void* stream);
 HMPC_EXTERNC int hmpc_predict_batch(hmpc_ctx* ctx, const struct update_data_t* in, int B, const unsigned char* mask,
                                     const double* wrench, double* pred_out);
+/* The certificate: a first-order optimality (KKT) check of robot i's wrench for its row, made on the device without the
+ * solve, so it judges any wrench: the solver's, qpOASES', a learned policy's.  The status word is not read.  From the row
+ * and the context's dt and f_max (hmpc_set_problem) it rebuilds the solve's float32 x0, Acd, Bcd and constraint rows
+ * (the same code computes them), runs the plan in float64, and takes the gradient of the QP objective by an adjoint sweep
+ * over it.  Per stance (step, leg) the rows within rounding of a bound are fitted to the gradient with sign-constrained
+ * multipliers; a swing leg's entries must be exactly 0.  DESIGN.md §3 gives the operations, §7 the thresholds.
+ *   cost              J = sum_k (x_k - traj_k)' S (x_k - traj_k) + u_k' Alpha_K u_k: the QP objective 1/2 U'HU + g'U plus
+ *                     the constant d'Sd of the record, float64 in a fixed order;
+ *   stationarity      max |grad J - A'lambda| over the largest gradient entry formed from absolute values (|x|, |u|, |S|,
+ *                     |Acd|, |Bcd|) of the stance legs;
+ *   primal            the worst bound violation or non-zero swing entry over the largest sum |a||u| of the stance rows;
+ *   complementarity   max |lambda| slack over the product of both scales;
+ *   n_active          the rows taken as active (candidates for a multiplier);
+ *   flags             HMPC_CERT_PASS alone when the inputs are finite, no swing entry is non-zero and each measure is
+ *                     within its threshold; otherwise the bits of what failed.
+ *   - lambda (NULL: not written) [B][N][2][8]: one per row of Fblk, >= 0 at a lower bound, <= 0 at an upper one, 0 on the
+ *     other rows and on swing legs: how hard each foot presses on its friction rows and force limit, the sensitivity of
+ *     the optimum to those bounds.  Where several rows are active at one point (a foot at zero force) it is one of many.
+ *   - A mask (NULL: every robot) skips robots with mask[i] == 0: their certificates and multipliers keep their bytes.
+ *   - Argument checks: a NULL context or pointer (lambda may be NULL) and B > capacity are HMPC_ERR_ARG; B = 0 is a no-op.
+ *   hmpc_certify_device: d_records B packed records, d_wrench [B][12N] float, d_mask NULL or device bytes [B], d_cert [B],
+ *                        d_lambda float.  One launch on `stream`, no host synchronisation.  Capturable.
+ *   hmpc_certify_batch : in B update_data_t, wrench [B][12N] double as the host solves return them, mask NULL or host bytes,
+ *                        lambda_out double.  In place when in, wrench, cert_out and lambda_out lie in pinned ranges
+ *                        (hmpc_pin_host_buffer), else staged through the context's pinned memory; the same results. */
+typedef struct hmpc_certificate_t {
+  double cost, stationarity, primal, complementarity;
+  int n_active, flags;
+} hmpc_certificate_t;
+#define HMPC_CERT_PASS 1          /* the wrench is a KKT point of its record's QP to the thresholds below */
+#define HMPC_CERT_NONFINITE 2     /* a non-finite wrench entry, state, gradient or row */
+#define HMPC_CERT_SWING 4         /* a swing leg's wrench entry is not 0 */
+#define HMPC_CERT_STATIONARITY 8  /* stationarity > HMPC_CERT_STATIONARITY_TOL */
+#define HMPC_CERT_PRIMAL 16       /* primal > HMPC_CERT_PRIMAL_TOL */
+#define HMPC_CERT_COMPLEMENTARITY 32  /* complementarity > HMPC_CERT_COMPLEMENTARITY_TOL */
+#define HMPC_CERT_STATIONARITY_TOL 2e-6
+#define HMPC_CERT_PRIMAL_TOL 2e-7
+#define HMPC_CERT_COMPLEMENTARITY_TOL 1e-9
+HMPC_EXTERNC int hmpc_certify_device(hmpc_ctx* ctx, const void* d_records, int B, const unsigned char* d_mask,
+                                     const float* d_wrench, hmpc_certificate_t* d_cert, float* d_lambda, void* stream);
+HMPC_EXTERNC int hmpc_certify_batch(hmpc_ctx* ctx, const struct update_data_t* in, int B, const unsigned char* mask,
+                                    const double* wrench, hmpc_certificate_t* cert_out, double* lambda_out);
 /* The reference boundary warm-started: after hmpc_reference_set_warm_start(1), every update_problem_data proposes the
  * previous call's working set moved one step (a hmpc_solve_batch_warm with shift NULL on the one-robot context).
  * setup_problem with another dt, f_max or horizon forgets it.  Default 0: every tick a cold start, like the reference. */
@@ -402,7 +444,7 @@ HMPC_EXTERNC int hmpc_swing_device(hmpc_ctx* ctx, const struct hmpc_state_t* d_s
 /* CUDA graphs.  The device-resident calls can be recorded into a CUDA graph by stream capture (cudaStreamBeginCapture,
  * torch.cuda.graph, ...) on the stream they are given: hmpc_solve_device, hmpc_solve_device_ex, hmpc_solve_device_warm,
  * hmpc_solve_device_masked, hmpc_solve_states_device_masked, hmpc_prepare_device, hmpc_rollout_device, hmpc_swing_device,
- * hmpc_predict_device and hmpc_reset_warm_start.  Each
+ * hmpc_predict_device, hmpc_certify_device and hmpc_reset_warm_start.  Each
  * launch of the graph gives the results an eager call on the same inputs gives, bit for bit.
  *   - A replay is a real call.  A captured warm solve proposes and records working sets, a captured rollout advances
  *     d_states and d_loop, a captured hmpc_reset_warm_start clears the working sets, every time the graph is launched.
@@ -414,7 +456,7 @@ HMPC_EXTERNC int hmpc_swing_device(hmpc_ctx* ctx, const struct hmpc_state_t* d_s
  *   - A call that returns an error while its stream is capturing may have recorded part of its work: end the capture
  *     and discard the graph.  Argument errors are found before anything is enqueued.
  * The host-buffer calls (hmpc_solve_batch, _ex, _warm, _masked, _states, _states_warm, _states_masked,
- * hmpc_solve_batch_sharded, hmpc_predict_batch) and the reference boundary
+ * hmpc_solve_batch_sharded, hmpc_predict_batch, hmpc_certify_batch) and the reference boundary
  * (update_problem_data) wait for their own streams and cannot be captured. */
 
 /* Robots beyond the conditioning limit (INTEGRATION.md).  The fp64 sweep inversion of the solve is accurate up to a scaled
