@@ -140,6 +140,12 @@ struct hmpc_ctx {
   // refinement class (hmpc_set_refinement): instances beyond the conditioning limit are solved again with iterative
   // refinement against the stored Hessian instead of ending with code 4
   ClassCfg ref{};
+  // the multi-query instantiations of the same classes (hmpc_solve_device_multi) and their scratch: d_mq + mq_off[c] for
+  // class c (3: the refinement class), one row of hmpc::mq_scratch_floats per CTA
+  ClassCfg mcls[3], mref{};
+  float* d_mq = nullptr;
+  size_t mq_off[4] = {};
+  unsigned char* h_multi = nullptr;  // pinned, max_batch x (row, traj, wrench, status, cost) of a staged hmpc_solve_batch_multi
   int* d_ref = nullptr;            // host-buffer path: [NCHUNK][1 + max_batch] refinement list length + list
   unsigned char* d_rec = nullptr;
   unsigned char* d_out = nullptr;  // host-buffer path: result staging (rows())
@@ -205,15 +211,19 @@ cudaError_t prep_class(const ClassCfg& c, int* occ)
   // The attribute is per kernel instantiation and process-wide, and several contexts (other horizons, the
   // reference-style global context) share the runtime-horizon instantiations: always raise it to the device's opt-in
   // maximum instead of this context's carve-up, so no context can lower it under another's launches.
-#define HMPC_PREP(ID, NT, MB, NF, CL)                                                                   \
+#define HMPC_PREP(ID, NT, MB, NF, CL) HMPC_PREP_K(ID, (hmpc::hmpc_solve_kernel<NT, MB, NF, CL>), NT)
+#define HMPC_PREP_MQ(ID, NT, MB, NF, CL) HMPC_PREP_K(ID, (hmpc::hmpc_solve_kernel<NT, MB, NF, CL, true>), NT)
+#define HMPC_PREP_K(ID, KERNEL, NT)                                                                    \
   case ID: {                                                                                           \
-    auto k = hmpc::hmpc_solve_kernel<NT, MB, NF, CL>;                                                  \
+    auto k = KERNEL;                                                                                   \
     e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);              \
     if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, k, NT, c.smem);       \
     break;                                                                                             \
   }
-  switch (c.variant) { HMPC_VARIANTS(HMPC_PREP) }
+  switch (c.variant) { HMPC_VARIANTS(HMPC_PREP) HMPC_MQ_VARIANTS(HMPC_PREP_MQ) }
 #undef HMPC_PREP
+#undef HMPC_PREP_MQ
+#undef HMPC_PREP_K
   return e;
 }
 
@@ -242,36 +252,54 @@ cudaError_t launch_chain(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t
   return cudaLaunchKernelEx(&cfg, kernel, args...);
 }
 
-// the shapes of the context's classes (hmpc::plan_classes) and what the device makes of them: resident CTAs per class
+// the shapes of the context's classes (hmpc::plan_classes) and what the device makes of them: resident CTAs per class;
+// the same for the multi-query classes, and their scratch
 int build_classes(hmpc_ctx* c)
 {
   c->ncls = hmpc::plan_classes(c->horizon, c->cls, c->ref);
-  if (c->ncls == 0) { g_err = "horizon too long for the built kernel variants"; return HMPC_ERR_ARG; }
-  for (int i = 0; i <= c->ncls; i++) {
-    ClassCfg& k = i < c->ncls ? c->cls[i] : c->ref;
+  if (c->ncls == 0 || hmpc::plan_classes(c->horizon, c->mcls, c->mref, true) != c->ncls) {
+    g_err = "horizon too long for the built kernel variants";
+    return HMPC_ERR_ARG;
+  }
+  size_t mq_rows = 0;
+  for (int i = 0; i <= 2 * c->ncls + 1; i++) {
+    const bool mq = i > c->ncls;
+    const int j = mq ? i - c->ncls - 1 : i;
+    ClassCfg& k = mq ? (j < c->ncls ? c->mcls[j] : c->mref) : (j < c->ncls ? c->cls[j] : c->ref);
     int occ = 0;
     if (cuda_fail(prep_class(k, &occ), "kernel attribute/occupancy (is this an sm_90a device?)")) return HMPC_ERR_CUDA;
     if (occ < 1) { g_err = "kernel does not fit on this device"; return HMPC_ERR_CUDA; }
     k.grid_cap = occ * c->sm_count;
+    if (mq) {
+      c->mq_off[j < c->ncls ? j : 3] = mq_rows * hmpc::mq_scratch_floats(c->horizon);
+      mq_rows += hmpc::mq_scratch_ctas(k, c->max_batch);
+    }
   }
+  if (cuda_fail(cudaMalloc(&c->d_mq, mq_rows * hmpc::mq_scratch_floats(c->horizon) * sizeof(float)), "cudaMalloc multi-query scratch"))
+    return HMPC_ERR_CUDA;
   return HMPC_OK;
 }
 
 long long* g_dbg_clk = nullptr;  // profiling hook (hmpc_debug_set_clock_buffer)
 
-// one launch of class `cls` (0-2, or hmpc::REFINE_CLASS) over `count` instances, as many CTAs as are resident at most
+// one launch of class `cls` (0-2, or hmpc::REFINE_CLASS) over `count` instances, as many CTAs as are resident at most;
+// with `mq` the class's multi-query instantiation
 int launch_class(const hmpc_ctx* c, int cls, const hmpc::SolveIO& io, const hmpc::ChainLists& lists, int count, cudaStream_t st,
-                 bool pdl = false)
+                 bool pdl = false, const hmpc::MultiIO* mq = nullptr)
 {
-  const ClassCfg& k = cls == hmpc::REFINE_CLASS ? c->ref : c->cls[cls];
-  hmpc::KernelArgs ka = hmpc::launch_args(c->cfg, c->horizon, c->ncls, cls, k, io, lists);
+  const ClassCfg& k = cls == hmpc::REFINE_CLASS ? (mq ? c->mref : c->ref) : (mq ? c->mcls[cls] : c->cls[cls]);
+  hmpc::KernelArgs ka = mq ? hmpc::multi_launch_args(c->cfg, c->horizon, c->ncls, cls, k, io, lists, *mq)
+                           : hmpc::launch_args(c->cfg, c->horizon, c->ncls, cls, k, io, lists);
   ka.dbg_clk = ka.dbg_H ? nullptr : g_dbg_clk;  // (the assembly dump is not stamped)
   const int grid = count < k.grid_cap ? count : k.grid_cap;
   cudaError_t e = cudaErrorInvalidDeviceFunction;
 #define HMPC_LAUNCH(ID, NT, MB, NF, CL) \
   case ID: e = launch_chain(hmpc::hmpc_solve_kernel<NT, MB, NF, CL>, dim3(grid), dim3(NT), (size_t)k.smem, st, pdl, ka); break;
-  switch (k.variant) { HMPC_VARIANTS(HMPC_LAUNCH) }
+#define HMPC_LAUNCH_MQ(ID, NT, MB, NF, CL) \
+  case ID: e = launch_chain(hmpc::hmpc_solve_kernel<NT, MB, NF, CL, true>, dim3(grid), dim3(NT), (size_t)k.smem, st, pdl, ka); break;
+  switch (k.variant) { HMPC_VARIANTS(HMPC_LAUNCH) HMPC_MQ_VARIANTS(HMPC_LAUNCH_MQ) }
 #undef HMPC_LAUNCH
+#undef HMPC_LAUNCH_MQ
   CK(e);
   CK(cudaGetLastError());
   return HMPC_OK;
@@ -314,6 +342,17 @@ int launch_certify(const hmpc_ctx* c, const void* rows, hmpc::RowLayout lay, int
   hmpc::hmpc_certify_kernel<T><<<hmpc::certify_grid(B), hmpc::CERT_THREADS, 0, st>>>(
       static_cast<const unsigned char*>(rows), lay, B, c->horizon, c->cfg.dt, c->cfg.f_max, mask, wrench,
       reinterpret_cast<hmpc::CertOut*>(cert), lambda, nullptr);
+  CK(cudaGetLastError());
+  return HMPC_OK;
+}
+
+// the multi-query call's cost kernel (hmpc_chain.h: multi_cost_grid) over the B x K rows
+template <typename T>
+int launch_multi_cost(const hmpc_ctx* c, const void* rows, hmpc::RowLayout lay, int B, int K, const unsigned char* mask,
+                      const float* traj, const T* wrench, double* cost, cudaStream_t st)
+{
+  hmpc::hmpc_multi_cost_kernel<T><<<hmpc::multi_cost_grid((long long)B * K), hmpc::PREDICT_THREADS, 0, st>>>(
+      static_cast<const unsigned char*>(rows), lay, B, K, c->horizon, c->cfg.dt, mask, traj, wrench, cost);
   CK(cudaGetLastError());
   return HMPC_OK;
 }
@@ -483,6 +522,8 @@ HMPC_EXTERNC void hmpc_destroy(hmpc_ctx* c)
   if (c->d_lists) cudaFree(c->d_lists);
   if (c->d_cls) cudaFree(c->d_cls);
   if (c->d_ref) cudaFree(c->d_ref);
+  if (c->d_mq) cudaFree(c->d_mq);
+  if (c->h_multi) cudaFreeHost(c->h_multi);
   shard_release(c);
   if (c->d_ws) cudaFree(c->d_ws);
   if (c->d_shift) cudaFree(c->d_shift);
@@ -597,7 +638,9 @@ namespace {
 // replays the lengths it was recorded with and nothing zeroes them between replays, so a chain recorded into a graph
 // uses the capture slot, starts with a memset node that zeroes both parities (the wave-barrier counter and the
 // refinement list length included), and leaves the eager call count alone.
-int enqueue_solve(hmpc_ctx* c, const hmpc::SolveIO& io, cudaStream_t st)
+// With `mq`, the multi-query instantiations of the classes run the chain (hmpc_chain.h: MultiIO): class 0 over the robots,
+// the later classes over lists of up to io.batch * K candidates.
+int enqueue_solve(hmpc_ctx* c, const hmpc::SolveIO& io, cudaStream_t st, const hmpc::MultiIO* mq = nullptr)
 {
   if (io.batch > c->max_batch) { g_err = "batch exceeds the context's capacity"; return HMPC_ERR_ARG; }
   CK(cudaSetDevice(c->device));
@@ -621,10 +664,11 @@ int enqueue_solve(hmpc_ctx* c, const hmpc::SolveIO& io, cudaStream_t st)
     // the states chain: records of the listed robots (every robot without a mask) into io.records, read by class 0
     if (int rc = launch_prepare(hmpc::prepare_args(c->horizon, io, lists), st, pdl)) return rc;
   }
+  const int items = mq ? io.batch * mq->K : io.batch;
   for (int i = 0; i < c->ncls; i++)
-    if (int rc = launch_class(c, i, io, lists, io.batch, st, pdl)) return rc;
+    if (int rc = launch_class(c, i, io, lists, i == 0 ? io.batch : items, st, pdl, mq)) return rc;
   // the refinement class at the end of the chain: exits at once when nobody was handed over
-  if (c->cfg.refine) return launch_class(c, hmpc::REFINE_CLASS, io, lists, io.batch, st, pdl);
+  if (c->cfg.refine) return launch_class(c, hmpc::REFINE_CLASS, io, lists, items, st, pdl, mq);
   return HMPC_OK;
 }
 
@@ -974,6 +1018,115 @@ HMPC_EXTERNC int hmpc_certify_batch(hmpc_ctx* c, const update_data_t* in, int B,
       if (lambda_out) memcpy(lambda_out + i * nl, hl + i * nl, nl * sizeof(double));
     }
   return HMPC_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// several reference trajectories per robot (hmpc_chain.h: MultiIO)
+// ---------------------------------------------------------------------------------------------------
+static int check_multi(const hmpc_ctx* c, int B, int K, const char* who)
+{
+  if (B < 0 || K < 1 || (long long)B * K > c->max_batch) {
+    g_err = std::string(who) + ": bad argument (B < 0, K < 1 or B*K > capacity)";
+    return HMPC_ERR_ARG;
+  }
+  return HMPC_OK;
+}
+
+static hmpc::MultiIO multi_io(const hmpc_ctx* c, const float* traj, int K)
+{
+  hmpc::MultiIO mq;
+  mq.traj = traj;
+  mq.K = K;
+  for (int i = 0; i < 4; i++) mq.scratch[i] = c->d_mq + c->mq_off[i];
+  return mq;
+}
+
+HMPC_EXTERNC int hmpc_solve_device_multi(hmpc_ctx* c, const void* d_records, int B, int K, const float* d_traj,
+                                         const unsigned char* d_mask, float* d_wrench, int* d_status, double* d_cost,
+                                         void* stream)
+{
+  if (!c || !d_records || !d_traj || !d_wrench || !d_status) { g_err = "hmpc_solve_device_multi: null argument"; return HMPC_ERR_ARG; }
+  if (int rc = check_multi(c, B, K, "hmpc_solve_device_multi")) return rc;
+  if (B == 0) return HMPC_OK;
+  if (int rc = check_device_records(c, d_records, B, "hmpc_solve_device_multi")) return rc;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  hmpc::SolveIO io = device_call(c, d_records, B, d_wrench, d_status, nullptr, false);
+  io.mask = d_mask;
+  const hmpc::MultiIO mq = multi_io(c, d_traj, K);
+  if (int rc = enqueue_solve(c, io, st, &mq)) return rc;
+  if (!d_cost) return HMPC_OK;
+  return launch_multi_cost(c, d_records, hmpc::packed_rows(c->horizon), B, K, d_mask, d_traj, d_wrench, d_cost, st);
+}
+
+namespace { int g_multi_in_place = -1; }
+HMPC_EXTERNC int hmpc_debug_last_multi_in_place(void) { return g_multi_in_place; }
+
+// The device-resident chain in the in-place mode (the kernels gather the update_data_t rows and store double wrenches), on the
+// caller's arrays when they are pinned, else on copies of the listed robots' rows in h_multi, which the kernels read mapped.
+HMPC_EXTERNC int hmpc_solve_batch_multi(hmpc_ctx* c, const update_data_t* in, int B, int K, const float* traj,
+                                        const unsigned char* mask, double* wrench_out, int* status, double* cost_out)
+{
+  if (!c || !in || !traj || !wrench_out || !status) { g_err = "hmpc_solve_batch_multi: null argument"; return HMPC_ERR_ARG; }
+  if (int rc = check_multi(c, B, K, "hmpc_solve_batch_multi")) return rc;
+  if (B == 0) return HMPC_OK;
+  if (mask && std::all_of(mask, mask + B, [](unsigned char m) { return m == 0; })) return HMPC_OK;
+  CK(cudaSetDevice(c->device));
+  const size_t nw = (size_t)12 * c->horizon, R = (size_t)B * K, mb = (size_t)c->max_batch;
+  const unsigned char* m = nullptr;
+  if (mask) {
+    memcpy(c->h_mask, mask, (size_t)B);  // pinned: the selection kernel and the cost kernel read it mapped
+    m = c->h_mask;
+  }
+  auto listed = [&](int i) { return !mask || mask[i] != 0; };
+  const bool in_place = c->pinned(in, (size_t)B * sizeof(update_data_t)) && c->pinned(traj, R * nw * sizeof(float)) &&
+                        c->pinned(wrench_out, R * nw * sizeof(double)) && c->pinned(status, R * sizeof(int)) &&
+                        (!cost_out || c->pinned(cost_out, R * sizeof(double)));
+  g_multi_in_place = in_place ? 1 : 0;
+  const update_data_t* rows = in;
+  const float* tr = traj;
+  double* w = wrench_out;
+  int* st = status;
+  double* cost = cost_out;
+  if (!in_place) {  // [max_batch rows | max_batch x 12N traj floats | ... wrench doubles | status ints | cost doubles]
+    if (!c->h_multi)
+      CK(cudaMallocHost(&c->h_multi, mb * (sizeof(update_data_t) + nw * (sizeof(float) + sizeof(double)) + sizeof(int) + sizeof(double))));
+    update_data_t* hr = reinterpret_cast<update_data_t*>(c->h_multi);
+    float* ht = reinterpret_cast<float*>(hr + mb);
+    double* hw = reinterpret_cast<double*>(ht + mb * nw);
+    double* hc = hw + mb * nw;
+    int* hs = reinterpret_cast<int*>(hc + mb);
+    for (int i = 0; i < B; i++)
+      if (listed(i)) {
+        hr[i] = in[i];
+        memcpy(ht + (size_t)i * K * nw, traj + (size_t)i * K * nw, K * nw * sizeof(float));
+      }
+    rows = hr, tr = ht, w = hw, st = hs, cost = cost_out ? hc : nullptr;
+  }
+  hmpc::SolveIO io;
+  io.raw = rows;
+  io.batch = B;
+  io.wrench64 = w;
+  io.status = st;
+  io.mask = m;
+  const hmpc::MultiIO mq = multi_io(c, tr, K);
+  if (int rc = enqueue_solve(c, io, c->stream, &mq)) return rc;
+  if (cost)
+    if (int rc = launch_multi_cost(c, rows, hmpc::update_rows(), B, K, m, tr, w, cost, c->stream)) return rc;
+  CK(cudaStreamSynchronize(c->stream));
+  int rc = HMPC_OK;
+  for (int i = 0; i < B; i++) {
+    if (!listed(i)) continue;
+    const size_t r0 = (size_t)i * K;
+    if (!in_place) {
+      memcpy(wrench_out + r0 * nw, w + r0 * nw, K * nw * sizeof(double));
+      memcpy(status + r0, st + r0, K * sizeof(int));
+      if (cost_out) memcpy(cost_out + r0, cost + r0, K * sizeof(double));
+    }
+    for (int k = 0; k < K; k++)
+      if (HMPC_STATUS_CODE(status[r0 + k]) != 0) rc = HMPC_ERR_NOT_CONVERGED;
+  }
+  if (rc) g_err = "hmpc_solve_batch_multi: at least one candidate did not reach a KKT point (see status[])";
+  return rc;
 }
 
 HMPC_EXTERNC int hmpc_pin_host_buffer(hmpc_ctx* c, void* ptr, size_t bytes)

@@ -17,6 +17,8 @@ namespace hmpc {
 //        register budget of 72 spills more and the 1024-robot batch was slower on the H100; class 1: 8 warps)
 //   10 + 5*cls + b: runtime horizon, b-th entry of {64, 128, 192, 256, 384} threads (class 2 runs class 1's kernel)
 //   20 + b: the refinement class, the same thread counts (one CTA per SM: it is rare and its shared memory is large)
+//   MQ_VARIANT + v (HMPC_MQ_VARIANTS): the multi-query instantiation of variant v (hmpc_solve_device_multi), the same shape
+constexpr int MQ_VARIANT = 100;
 #define HMPC_VARIANTS(X) \
   X(0, 128, 6, 10, 0)    \
   X(1, 256, 2, 10, 1)    \
@@ -35,6 +37,24 @@ namespace hmpc {
   X(17, 192, 3, 0, 1)    \
   X(18, 256, 2, 0, 1)    \
   X(19, 384, 1, 0, 1)
+#define HMPC_MQ_VARIANTS(X) \
+  X(100, 128, 6, 10, 0) \
+  X(101, 256, 2, 10, 1) \
+  X(120, 64, 1, 0, 3)   \
+  X(121, 128, 1, 0, 3)  \
+  X(122, 192, 1, 0, 3)  \
+  X(123, 256, 1, 0, 3)  \
+  X(124, 384, 1, 0, 3)  \
+  X(110, 64, 8, 0, 0)   \
+  X(111, 128, 6, 0, 0)  \
+  X(112, 192, 3, 0, 0)  \
+  X(113, 256, 2, 0, 0)  \
+  X(114, 384, 1, 0, 0)  \
+  X(115, 64, 8, 0, 1)   \
+  X(116, 128, 6, 0, 1)  \
+  X(117, 192, 3, 0, 1)  \
+  X(118, 256, 2, 0, 1)  \
+  X(119, 384, 1, 0, 1)
 
 constexpr int REFINE_CLASS = 3;           // kernel class of the refinement class
 constexpr int SMEM_MAX = 226 * 1024;      // dynamic shared memory a class may take (the H100's opt-in maximum is 227 KB)
@@ -46,8 +66,8 @@ struct ClassCfg {
 };
 
 // The variant of kernel class `kcls` at horizon N: the one fixed at N when `fixed` allows it, else the runtime-horizon one
-// with the fewest threads that still give `warps` warps.  -1 when there is none.
-inline int pick_variant(int N, int kcls, int warps, bool fixed, int* threads)
+// with the fewest threads that still give `warps` warps; multi-query instantiations when `mq`.  -1 when there is none.
+inline int pick_variant(int N, int kcls, int warps, bool fixed, int* threads, bool mq = false)
 {
   int v = -1;
 #define HMPC_PICK(ID, NT, MB, NF, CL) \
@@ -58,7 +78,7 @@ inline int pick_variant(int N, int kcls, int warps, bool fixed, int* threads)
   if (CL == kcls && NF == N && fixed && v >= 0) v = ID, *threads = NT;
   HMPC_VARIANTS(HMPC_PICK)
 #undef HMPC_PICK
-  return v;
+  return (v >= 0 && mq) ? MQ_VARIANT + v : v;
 }
 
 // Shapes of classes 0-2 (cls) and of the refinement class (ref) at horizon N.  Returns the number of size classes, 2 when
@@ -71,14 +91,15 @@ inline int pick_variant(int N, int kcls, int warps, bool fixed, int* threads)
 //   refinement: class 2's shape plus the float32 H tiles and g its refinement rounds read (refine_layout).  It holds
 //            double support (2N blocks) while that leaves at least class 1's working-set capacity, i.e. up to horizon 14;
 //            beyond that single support (N blocks), and an instance with more stance blocks keeps its code 4.
-inline int plan_classes(int N, ClassCfg cls[3], ClassCfg& ref)
+// mq: the multi-query instantiations of the same shapes (hmpc_solve_device_multi).
+inline int plan_classes(int N, ClassCfg cls[3], ClassCfg& ref, bool mq = false)
 {
   const int rs = record_stride(N);
   for (int i = 0; i < 2; i++) {
     ClassCfg& k = cls[i];
     k = ClassCfg{};
     k.nb_cap = k.nb_hi = class_nb_cap(N, i);
-    k.variant = pick_variant(N, i, class_warps(N, i), true, &k.threads);
+    k.variant = pick_variant(N, i, class_warps(N, i), true, &k.threads, mq);
     if (k.variant < 0) return 0;
     k.qmax = class_qmax(N, i);
     k.tcap = class_tcap(N, i);
@@ -87,7 +108,7 @@ inline int plan_classes(int N, ClassCfg cls[3], ClassCfg& ref)
   }
   ClassCfg& k = cls[2];
   k = cls[1];
-  k.variant = pick_variant(N, 1, class_warps(N, 1), false, &k.threads);  // (a fixed variant folds class 1's layout)
+  k.variant = pick_variant(N, 1, class_warps(N, 1), false, &k.threads, mq);  // (a fixed variant folds class 1's layout)
   k.qmax = 6 * k.nb_cap;
   k.tcap = 0;
   k.L = make_layout(N, k.nb_cap, k.qmax, rs, k.threads / 32, 0);
@@ -100,7 +121,7 @@ inline int plan_classes(int N, ClassCfg cls[3], ClassCfg& ref)
   for (int nb = 2 * N;; nb = N) {
     ref = ClassCfg{};
     ref.nb_cap = ref.nb_hi = nb;
-    ref.variant = pick_variant(N, REFINE_CLASS, class_warps(N, nb == N ? 0 : 1), false, &ref.threads);
+    ref.variant = pick_variant(N, REFINE_CLASS, class_warps(N, nb == N ? 0 : 1), false, &ref.threads, mq);
     if (ref.variant < 0) return 0;
     ref.qmax = 6 * nb;
     ref.L = refine_layout(N, nb, ref.qmax, rs, ref.threads / 32);
@@ -337,6 +358,40 @@ inline KernelArgs launch_args(const SolverSettings& S, int N, int ncls, int cls,
   ka.tau = io.tau;
   ka.L = k.L;
   return ka;
+}
+
+// A multi-query call (hmpc_solve_device_multi): the chain of hmpc_solve_device over the io.batch robots with the multi-query
+// classes (plan_classes(..., mq = true)), K candidate trajectories per robot (traj [batch][K][12N]) and results in rows
+// i*K + k of io.wrench / io.wrench64 / io.status.  Calls are cold: no working set is proposed or recorded, and no torques.
+// scratch[c]: class c's scratch (REFINE_CLASS: scratch[3]), mq_scratch_floats(N) floats per CTA of its launch.
+struct MultiIO {
+  const float* traj = nullptr;
+  int K = 1;
+  float* scratch[4] = {};
+};
+inline KernelArgs multi_launch_args(const SolverSettings& S, int N, int ncls, int cls, const ClassCfg& k, const SolveIO& io,
+                                    const ChainLists& lists, const MultiIO& mq)
+{
+  KernelArgs ka = launch_args(S, N, ncls, cls, k, io, lists);
+  ka.warm_start = 0;
+  ka.ws_state = nullptr;
+  ka.ws_shifts = nullptr;
+  ka.tau = nullptr;
+  ka.mq_traj = mq.traj;
+  ka.mq_k = mq.K;
+  ka.mq_scratch = mq.scratch[cls == REFINE_CLASS ? 3 : cls];
+  return ka;
+}
+// CTAs a class's multi-query scratch serves: its launches have at most grid_cap CTAs, and a class's list holds at most
+// max_batch entries
+inline size_t mq_scratch_ctas(const ClassCfg& k, int max_batch) { return (size_t)(k.grid_cap < max_batch ? k.grid_cap : max_batch); }
+
+// The multi-query call's cost launch (hmpc_multi_cost_kernel): one warp per result row, multi_cost_grid(batch * K) CTAs of
+// PREDICT_THREADS, behind the chain in plain stream order.
+inline int multi_cost_grid(long long nrows)
+{
+  constexpr int warps = PREDICT_THREADS / 32;
+  return (int)((nrows + warps - 1) / warps);
 }
 
 }  // namespace hmpc

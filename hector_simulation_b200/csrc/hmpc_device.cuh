@@ -191,7 +191,15 @@ struct KernelArgs {
   float* tau;                    // [batch][10] joint torques of the first-step wrench (row f-2), or nullptr
   long long* dbg_clk;            // [batch][32] stage timestamps (clock64) of thread 0, profiling hook; null in production
   Layout L;
+  // multi-query launches (hmpc_solve_kernel<..., MQ = true>): K reference trajectories per robot, results in row i*K + k
+  const float* mq_traj;          // [batch][K][12N] the candidates' trajectories (the record's own traj is not used)
+  int mq_k;                      // K
+  float* mq_scratch;             // [gridDim.x][mq_scratch_floats(N)]: what stage 2 of a CTA's robot leaves for its later candidates
 };
+
+// Multi-query scratch of one CTA, floats: x0 (16) | Acd (172) | Bcd (156) | the state weights (12) | M (72N).  Stage 5 reuses
+// the union these live in, so the later candidates of a robot read them back from here.
+__host__ __device__ constexpr int mq_scratch_floats(int N) { return 16 + 172 + 156 + 12 + 72 * N; }
 
 // ------------------------------------------------------------------------------------------------
 // small helpers
@@ -969,7 +977,17 @@ __global__ void hmpc_swing_kernel(const unsigned char* states, const unsigned ch
 #endif
 constexpr int WS_STATE_INTS = 40;  // persistent working set of one robot: [0] = count, then (step*2+leg) << 8 | normal index
 
-template <int NT, int MINB, int NF, int CLS>
+// A multi-query list entry: the robot, and its candidates [mq_first, mq_end).  Robots only (class 0), or candidates i*K + k and
+// whole robots -1 - i (the later classes: `items`).
+__device__ __forceinline__ int mq_robot(int ent, int K, bool items) { return !items ? ent : (ent < 0 ? -1 - ent : ent / K); }
+__device__ __forceinline__ int mq_first(int ent, int K, bool items) { return (items && ent >= 0) ? ent % K : 0; }
+__device__ __forceinline__ int mq_end(int ent, int K, bool items) { return (items && ent >= 0) ? ent % K + 1 : K; }
+
+// MQ (multi-query, hmpc_solve_device_multi): a CTA takes a robot through stages 0-4 once and then runs the rest of the solve
+// (the trajectory's d rows of stage 2, the gradient, stages 5-6) once per candidate trajectory k, into result row i*K + k.
+// The list of class 0 (or its identity) holds robots; the lists of classes 1-2 and of the refinement class hold candidates
+// i*K + k (escalated alone) or -1 - i (a robot class 0 classified out, with all K candidates).
+template <int NT, int MINB, int NF, int CLS, bool MQ = false>
 __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs ka)
 {
   extern __shared__ __align__(16) unsigned char smem[];
@@ -1066,7 +1084,11 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
       __syncthreads();
     }
     if (idx >= count) continue;  // the last wave may not fill the grid
-    const int inst = ka.list ? ka.list[idx] : idx;
+    // the robot (its record) and its candidates [k0, k1); one solve for every other launch
+    const int inst = MQ ? mq_robot(ka.list ? ka.list[idx] : idx, ka.mq_k, CLS == 3 || ka.cls > 0)
+                        : (ka.list ? ka.list[idx] : idx);
+    const int k0 = MQ ? mq_first(ka.list ? ka.list[idx] : idx, ka.mq_k, CLS == 3 || ka.cls > 0) : 0;
+    const int k1 = MQ ? mq_end(ka.list ? ka.list[idx] : idx, ka.mq_k, CLS == 3 || ka.cls > 0) : 1;
     HMPC_STAMP(0);
     // ---------------- stage 0: record -> shared memory (TMA bulk copy) ----------------
     const bool raw = ka.raw_records != nullptr;
@@ -1183,7 +1205,7 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
       // size classification folded into the launch: more stance blocks than this class holds -> next class's list
       if (tid == 0) {
         const int slot = atomicAdd(&ka.counts[ka.cls + 1], 1);
-        ka.esc_list[slot] = inst;
+        ka.esc_list[slot] = MQ ? -1 - inst : inst;  // (multi-query: the robot with all its candidates)
       }
       __syncthreads();
       continue;
@@ -1206,6 +1228,29 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
       nrm[e] = (double)(neg ? -v : v);
     }
 
+    // Multi-query: everything below runs once per candidate kq (the jump back at the end); stages 2-4 skip what does not
+    // depend on the trajectory after the first (the powers and Toeplitz blocks, H, the sweep), and H^-1 survives in place.
+    float* const mqs = MQ ? ka.mq_scratch + (size_t)blockIdx.x * mq_scratch_floats(N) : nullptr;
+    bool illc_h = false;  // the conditioning check of stage 5 (it reads the diagonal of H, which the first candidate spends)
+    int kq = k0;
+  next_candidate:
+    const bool first = kq == k0;
+    const int row = MQ ? inst * ka.mq_k + kq : inst;  // result row
+    const float* trj = MQ ? ka.mq_traj + (size_t)row * 12 * N : nullptr;  // the candidate's reference trajectory
+    if (MQ && !first) {
+      // the stage-2 operands and the weights, back from the scratch into the union (the previous candidate's stage 5 used it)
+      float* wts = reinterpret_cast<float*>(rec) + 30;
+      for (int e = tid; e < mq_scratch_floats(N); e += NT) {
+        const float v = mqs[e];
+        if (e < 16) x0f[e] = v;
+        else if (e < 16 + 172) { if (e < 16 + 169) Acd[e - 16] = v; }
+        else if (e < 344) Bcd[e - 188] = v;
+        else if (e < 356) wts[e - 344] = v;
+        else Mb[e - 356] = v;
+      }
+      __syncthreads();
+    }
+
     HMPC_STAMP(1);
     // ---------------- stage 2: powers of Acd, Toeplitz blocks, d = A_qp x0 - X_d ----------------
     // Acd = I + dt*A has the SRBD pattern (SolverMPC.cpp:312-318): Rb block (rows 0-2, cols 6-8), dt on
@@ -1219,6 +1264,7 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
     // Rows 6..11 of M_k equal Bcd's rows for every k and are read from Bcd directly by stage 3.
     for (int it = tid; it < 48; it += NT) {
       if (it < 36) {
+        if (MQ && !first) continue;
         const int r = it / 12, c = it % 12;
         const float a0 = Acd[r * 13 + 6], a1 = Acd[r * 13 + 7], a2 = Acd[r * 13 + 8], ad = Acd[(3 + r) * 13 + 9 + r];
         const float b6 = Bcd[6 * 12 + c], b7 = Bcd[7 * 12 + c], b8 = Bcd[8 * 12 + c], b9 = Bcd[(9 + r) * 12 + c];
@@ -1243,7 +1289,7 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
             p1 = FA(a1, p1);
             p2 = FA(a2, p2);
             const float acc = FA(FA(FA(xr_, FM(p0, x0f[6])), FM(p1, x0f[7])), FM(p2, x0f[8]));
-            dd[12 * s + r] = FS(acc, rf[54 + 12 * s + r]);
+            dd[12 * s + r] = FS(acc, (MQ ? trj[12 * s + r] : rf[54 + 12 * s + r]));
           }
         } else if (r < 6) {
           const float ad = Acd[r * 13 + r + 6], ag = Acd[11 * 13 + 12];
@@ -1253,7 +1299,7 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
             pd = FA(ad, pd);
             float acc = FA(xr_, FM(pd, x0f[r + 6]));
             if (r == 5) acc = FA(acc, FM(p5, x0f[12]));
-            dd[12 * s + r] = FS(acc, rf[54 + 12 * s + r]);
+            dd[12 * s + r] = FS(acc, (MQ ? trj[12 * s + r] : rf[54 + 12 * s + r]));
           }
         } else {
           const float ag = Acd[11 * 13 + 12];
@@ -1261,12 +1307,23 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
           for (int s = 0; s < N; s++) {
             p11 = FA(ag, p11);
             const float acc = (r == 11) ? FA(xr_, FM(p11, x0f[12])) : xr_;
-            dd[12 * s + r] = FS(acc, rf[54 + 12 * s + r]);
+            dd[12 * s + r] = FS(acc, (MQ ? trj[12 * s + r] : rf[54 + 12 * s + r]));
           }
         }
       }
     }
     __syncthreads();
+    if (MQ && first && k1 - k0 > 1) {
+      for (int e = tid; e < mq_scratch_floats(N); e += NT) {
+        float v = 0.f;
+        if (e < 16) v = x0f[e];
+        else if (e < 16 + 172) { if (e < 16 + 169) v = Acd[e - 16]; }
+        else if (e < 344) v = Bcd[e - 188];
+        else if (e < 356) v = rf[30 + e - 344];
+        else v = Mb[e - 356];
+        mqs[e] = v;
+      }
+    }
 
     HMPC_STAMP(2);
     // ---------------- stage 3: Hessian prefix chains (one 1x6 leg tile per item) + gradient ----------------
@@ -1293,7 +1350,7 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
       // item = (li, lj, delta, i): running sums G_delta(K)[i][leg lj's six columns] = sum_{e<=K} T_{e+delta}^T M_e;
       // block (a,b) of B'SB, b - a = delta, equals G_delta(N-1-b) — the oracle's own summation order.
       // 32-item chunks in list order (longest chains first) go to the warps round-robin.
-      const int nitems = flags[6] * 6;
+      const int nitems = (!MQ || first) ? flags[6] * 6 : 0;  // (H does not depend on the trajectory)
       for (int chunk = wid; chunk * 32 < nitems; chunk += NW) {
         const int it = chunk * 32 + lane;
         if (it >= nitems) continue;
@@ -1420,14 +1477,23 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
     if (dump) continue;
 
     if (NB == 0) {
-      for (int e = tid; e < 12 * N; e += NT) {
-        if (ka.wrench) ka.wrench[(size_t)inst * 12 * N + e] = 0.f;
-        if (ka.wrench64) ka.wrench64[(size_t)inst * 12 * N + e] = 0.0;
-      }
-      if (ka.tau && tid < 10) ka.tau[(size_t)inst * 10 + tid] = 0.f;
-      if (tid == 0) {
-        ka.status[inst] = ST_OK;
-        if (ka.ws_state) ka.ws_state[(size_t)inst * WS_STATE_INTS] = 0;
+      if constexpr (MQ) {  // every candidate at once
+        const size_t r0 = (size_t)inst * ka.mq_k + kq;
+        for (int e = tid; e < (k1 - kq) * 12 * N; e += NT) {
+          if (ka.wrench) ka.wrench[r0 * 12 * N + e] = 0.f;
+          if (ka.wrench64) ka.wrench64[r0 * 12 * N + e] = 0.0;
+        }
+        for (int e = tid; e < k1 - kq; e += NT) ka.status[r0 + e] = ST_OK;
+      } else {
+        for (int e = tid; e < 12 * N; e += NT) {
+          if (ka.wrench) ka.wrench[(size_t)inst * 12 * N + e] = 0.f;
+          if (ka.wrench64) ka.wrench64[(size_t)inst * 12 * N + e] = 0.0;
+        }
+        if (ka.tau && tid < 10) ka.tau[(size_t)inst * 10 + tid] = 0.f;
+        if (tid == 0) {
+          ka.status[inst] = ST_OK;
+          if (ka.ws_state) ka.ws_state[(size_t)inst * WS_STATE_INTS] = 0;
+        }
       }
       __syncthreads();
       continue;
@@ -1436,7 +1502,8 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
       // the exact QP data for the residuals of the refinement rounds: stage 4 inverts the tiles in place, gq becomes zb
       float* Hc = reinterpret_cast<float*>(smem + L.Hc);
       double* gc = reinterpret_cast<double*>(smem + L.gc);
-      for (int e = tid; e < tri(NT8) * 64; e += NT) Hc[e] = Hf[e];
+      if (!MQ || first)
+        for (int e = tid; e < tri(NT8) * 64; e += NT) Hc[e] = Hf[e];
       for (int e = tid; e < n; e += NT) gc[e] = gq[e];
     }
 
@@ -1449,7 +1516,7 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
     // whole stage.  Per block step: ONE barrier.  During step k the owners of panel k+1 update those tiles first and
     // publish them (the diagonal one already inverted, in-register) in fragment order, so that in step k+1 every
     // operand of W_I = P_I D^-1 and of the rank-8 updates A_IJ -= W_I P_J' is one conflict-free 8-byte load.
-    {
+    if (!MQ || first) {
       // accumulator slots: tile J of row rB in c[J], tile J of row rA in c[2NW - J] (rA + rB = NT8 - 1 <= 2NW - 1, so the
       // two never meet) — every slot index is a compile-time constant of the unrolled loops
       constexpr int TS = 2 * NW + 1;
@@ -1657,7 +1724,8 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
     bool illc = false;
     if (isvar) {
       xreg = -hinv_rowdot(Hd, vi, NT8, gq);
-      illc = x0[vi] * Hd[toff(vi >> 3, vi >> 3) + (vi & 7) * 9] > ka.kappa_max;
+      if (!MQ || first) illc_h = x0[vi] * Hd[toff(vi >> 3, vi >> 3) + (vi & 7) * 9] > ka.kappa_max;
+      illc = illc_h;
       x0[vi] = xreg;
     }
     {
@@ -2322,8 +2390,8 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
       const int s = e / 12, c12 = e % 12, leg = leg_of(c12);
       const int k = sl_blk[2 * s + leg];
       const double v = (k >= 0) ? zb[6 * k + loc_of(c12)] : 0.0;
-      if (ka.wrench) ka.wrench[(size_t)inst * 12 * N + e] = (float)v;
-      if (ka.wrench64) ka.wrench64[(size_t)inst * 12 * N + e] = v;
+      if (ka.wrench) ka.wrench[(size_t)row * 12 * N + e] = (float)v;
+      if (ka.wrench64) ka.wrench64[(size_t)row * 12 * N + e] = v;
     }
     if (ka.tau && tid < 10) {
       // row f-2: tau = J_force_moment^T * f_ff, f_ff = -rBody [F; M] of the first-step wrench
@@ -2357,17 +2425,20 @@ __global__ void __launch_bounds__(NT, MINB) hmpc_solve_kernel(const KernelArgs k
     if (tid == 0) {
       if (code == ST_WS_CAP && ka.esc_list) {  // hand over to the next class (larger working-set capacity)
         const int slot = atomicAdd(&ka.counts[ka.cls + 1], 1);
-        ka.esc_list[slot] = inst;
+        ka.esc_list[slot] = row;
       }
       if (code == ST_NOT_SPD && flags[3] == ST_OK && ka.ref_list) {  // beyond the conditioning limit, every pivot positive
         const int slot = atomicAdd(ka.ref_count, 1);
-        ka.ref_list[slot] = inst;
+        ka.ref_list[slot] = row;
       }
       int sw = (code & 0xff) | ((iters & 0xfff) << 8) | ((q & 0xff) << 20);
       if constexpr (CLS == 3) sw |= refined ? (1 << 28) : 0;  // HMPC_STATUS_REFINED
-      ka.status[inst] = sw;
+      ka.status[row] = sw;
     }
     __syncthreads();
+    if constexpr (MQ) {
+      if (++kq < k1) goto next_candidate;
+    }
   }
 }
 
@@ -2482,6 +2553,22 @@ struct PlanRow {
     return acc;
   }
 };
+
+// The tracking cost of a plan, J = sum_k (x_{k+1} - traj_k)' S (x_{k+1} - traj_k) + u_k' alpha u_k, in float64 on lane r < 12:
+// cost_step after each step of the recurrence (x = x_{k+1}[r], xd = traj_k[r], u = u_k[r]), then cost_total on the whole warp
+// adds the twelve lanes' sums in lane order.  The certificate's cost and the multi-query call's cost are these.
+__device__ __forceinline__ double cost_step(double cost, double S, double Al, double x, double xd, double u)
+{
+  const double e = DS(x, xd);
+  cost = DA(cost, DM(DM(S, e), e));
+  return DA(cost, DM(DM(Al, u), u));
+}
+__device__ __forceinline__ double cost_total(double cost)
+{
+  double J = 0.0;
+  for (int r = 0; r < 12; r++) J = DA(J, __shfl_sync(0xffffffffu, cost, r));
+  return J;
+}
 
 constexpr int PREDICT_THREADS = 128;
 constexpr int PREDICT_WARP_BYTES = 1440;  // per warp: role scratch 64 B | x0 16 floats | Acd 169 | Bcd 156 floats
@@ -2743,15 +2830,12 @@ __global__ void __launch_bounds__(CERT_THREADS) hmpc_certify_kernel(const unsign
         xa = na;
         X[12 * k + lane] = x;
         XA[12 * k + lane] = xa;
-        const double e = DS(x, (double)traj[12 * k + lane]);
-        cost = DA(cost, DM(DM(S, e), e));
-        cost = DA(cost, DM(DM(Al, u), u));
+        cost = cost_step(cost, S, Al, x, (double)traj[12 * k + lane], u);
         fin = fin && finite64(u) && finite64(x);
       }
     }
   }
-  double J = 0.0;
-  for (int r = 0; r < 12; r++) J = DA(J, __shfl_sync(0xffffffffu, cost, r));
+  const double J = cost_total(cost);
   __syncwarp();
 
   // ---- 3. the adjoint sweep and the gradient
@@ -2908,6 +2992,53 @@ __global__ void __launch_bounds__(CERT_THREADS) hmpc_certify_kernel(const unsign
     c.flags = f;
     cert[i] = c;
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// The cost of the multi-query call (hmpc_solve_device_multi, hmpc_solve_batch_multi): for row q = i*K + k, the certificate's
+// tracking cost J (cost_step, cost_total; hmpc_certify_kernel, step 2) of wrench row q on robot i's row of `rows` (layout
+// `lay`) with the reference trajectory traj[q] [12N] in place of the row's own.  One warp per row: stage 1's role_state and
+// role_inertia, then the plan's recurrence (PlanRow), as hmpc_predict_kernel runs them.  Robots with mask[i] == 0 (mask
+// non-null) are skipped.  T: the wrench's element type.  Launch shape: hmpc_chain.h, multi_cost_grid.
+// ------------------------------------------------------------------------------------------------
+template <typename T>
+__global__ void __launch_bounds__(PREDICT_THREADS) hmpc_multi_cost_kernel(const unsigned char* rows, RowLayout lay, int batch,
+                                                                           int K, int N, float dt, const unsigned char* mask,
+                                                                           const float* traj, const T* wrench, double* cost)
+{
+  constexpr int NW = PREDICT_THREADS / 32;
+  __shared__ __align__(16) unsigned char scratch[NW * PREDICT_WARP_BYTES];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const long long q = (long long)blockIdx.x * NW + wid;
+  if (q >= (long long)batch * K) return;  // (the whole warp)
+  const int i = (int)(q / K);
+  if (mask && mask[i] == 0) return;
+  unsigned char* scr = scratch + wid * PREDICT_WARP_BYTES;
+  float* x0f = reinterpret_cast<float*>(scr + 64);
+  float* Acd = x0f + 16;
+  float* Bcd = Acd + 169;  // (not zeroed: the roles write every entry read below)
+  const unsigned char* row = rows + (size_t)i * lay.stride;
+  const float* rf = reinterpret_cast<const float*>(row);
+  const float* alpha = reinterpret_cast<const float*>(row + lay.alpha);
+  const float* xd = traj + (size_t)q * 12 * N;
+  const T* w = wrench + (size_t)q * 12 * N;
+  role_state(rf, dt, x0f, Acd, lane, scr);
+  if (lane == 31) role_inertia(rf, dt, Bcd);
+  __syncwarp();
+  const PlanRow<false> pr(Acd, Bcd, lane);
+  const int j = lane < 12 ? lane : 0;
+  const double S = (double)rf[30 + j], Al = (double)alpha[j];
+  double x = lane < 13 ? (double)x0f[lane] : 0.0, c = 0.0;
+  for (int k = 0; k < N; k++) {
+    const double u = lane < 12 ? (double)w[12 * k + lane] : 0.0;
+    const double nx = pr.step(x, u);
+    if (lane < 12) {
+      x = nx;
+      c = cost_step(c, S, Al, x, (double)xd[12 * k + lane], u);
+    }
+  }
+  const double J = cost_total(c);
+  if (lane == 0) cost[q] = J;
 }
 
 }  // namespace hmpc

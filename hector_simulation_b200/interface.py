@@ -35,6 +35,7 @@ EXPORTS = [
     "hmpc_solve_states_device_masked", "hmpc_solve_batch_states_warm", "hmpc_solve_batch_states_masked",
     "hmpc_solve_batch_sharded_warm", "hmpc_solve_batch_states_sharded_warm",
     "hmpc_predict_device", "hmpc_predict_batch", "hmpc_certify_device", "hmpc_certify_batch",
+    "hmpc_solve_device_multi", "hmpc_solve_batch_multi",
 ]
 # hmpc_certificate_t, and its flag bits (include/hector_mpc_b200.h)
 CERTIFICATE_DTYPE = np.dtype([("cost", "<f8"), ("stationarity", "<f8"), ("primal", "<f8"), ("complementarity", "<f8"),
@@ -152,6 +153,10 @@ def lib() -> ctypes.CDLL:
         L.hmpc_certify_device.restype = ctypes.c_int
         L.hmpc_certify_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 4
         L.hmpc_certify_batch.restype = ctypes.c_int
+        L.hmpc_solve_device_multi.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 6
+        L.hmpc_solve_device_multi.restype = ctypes.c_int
+        L.hmpc_solve_batch_multi.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 5
+        L.hmpc_solve_batch_multi.restype = ctypes.c_int
         _lib = L
     return _lib
 
@@ -592,6 +597,48 @@ class BatchedMPC:
         _check(lib().hmpc_certify_batch(self._h, records.ctypes.data, B, m, wrench.ctypes.data, out.ctypes.data,
                                         lam.ctypes.data if want_lam else None))
         return (out, lam) if want_lam else out
+
+    def solve_device_multi(self, d_records, B: int, d_traj, d_wrench, d_status, d_cost=None, d_mask=None, stream=None) -> None:
+        """Robot i's MPC for K candidate reference trajectories at once (hmpc_solve_device_multi).  torch CUDA tensors:
+        records uint8 [B,stride]; d_traj f32 [B,K,12N] (laid out like the record's traj, which is not read); results d_wrench
+        f32 [B,K,12N], d_status i32 [B,K], d_cost f64 [B,K] or None: the tracking cost J of certify_device, for ranking the
+        candidates.  Candidate (i,k) equals solve_device on robot i's record with traj k, bit for bit.  `d_mask` bool or uint8
+        [B] or None: unlisted robots' rows keep their bytes.  Cold, enqueued on the current stream, capturable."""
+        import torch
+
+        K = d_traj.shape[1]
+        st = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        _check(lib().hmpc_solve_device_multi(self._h, d_records.data_ptr(), B, K, d_traj.data_ptr(),
+                                             d_mask.data_ptr() if d_mask is not None else None, d_wrench.data_ptr(),
+                                             d_status.data_ptr(), d_cost.data_ptr() if d_cost is not None else None,
+                                             ctypes.c_void_p(st)))
+
+    def solve_batch_multi(self, records: np.ndarray, traj: np.ndarray, mask=None, cost: bool = True, strict: bool = True,
+                          out=None):
+        """solve_device_multi from host buffers (hmpc_solve_batch_multi): `records` update_data_t [B], `traj` f32 [B,K,12N]
+        -> (wrench f64 [B,K,12N], status i32 [B,K], cost f64 [B,K] or None).  `out=(wrench, status, cost)` reuses the
+        caller's arrays (cost may be None); in place when records, traj and every output are pinned (pin()).  With a mask
+        only listed robots' rows are written.  strict: raise when a listed candidate did not converge."""
+        records = np.ascontiguousarray(records, dtype=UPDATE_DTYPE)
+        traj = np.ascontiguousarray(traj, dtype=np.float32)
+        B, N = records.shape[0], self.horizon
+        assert traj.ndim == 3 and traj.shape[0] == B and traj.shape[2] == 12 * N
+        K = traj.shape[1]
+        if out is None:
+            out = (np.zeros((B, K, 12 * N), np.float64), np.zeros((B, K), np.int32), np.zeros((B, K), np.float64) if cost else None)
+        w, st, c = out
+        assert w.dtype == np.float64 and w.shape == (B, K, 12 * N) and w.flags.c_contiguous
+        assert st.dtype == np.int32 and st.shape == (B, K) and st.flags.c_contiguous
+        assert c is None or (c.dtype == np.float64 and c.shape == (B, K) and c.flags.c_contiguous)
+        m = None
+        if mask is not None:
+            mask = np.ascontiguousarray(np.asarray(mask) != 0).view(np.uint8)
+            assert mask.shape == (B,)
+            m = mask.ctypes.data
+        _check(lib().hmpc_solve_batch_multi(self._h, records.ctypes.data, B, K, traj.ctypes.data, m, w.ctypes.data,
+                                            st.ctypes.data, c.ctypes.data if c is not None else None),
+               allow_not_converged=not strict)
+        return w, st, c
 
     def assemble_device(self, d_records, B: int, stream=None) -> dict:
         """Parity hook: un-reduced fp32 QP data of B packed records (torch tensors on the GPU)."""

@@ -361,6 +361,34 @@ HMPC_EXTERNC int hmpc_certify_device(hmpc_ctx* ctx, const void* d_records, int B
                                      const float* d_wrench, hmpc_certificate_t* d_cert, float* d_lambda, void* stream);
 HMPC_EXTERNC int hmpc_certify_batch(hmpc_ctx* ctx, const struct update_data_t* in, int B, const unsigned char* mask,
                                     const double* wrench, hmpc_certificate_t* cert_out, double* lambda_out);
+/* Several reference trajectories per robot: robot i's MPC solved for K candidate trajectories traj[i][k] [12N] (laid out
+ * like update_data_t::traj) at once.  The record's own traj bytes are not read; everything else in it is shared by the K
+ * candidates, so the QP's constraints, its Hessian and the sweep inversion are computed once per robot and only the
+ * gradient and the active-set stage run per candidate (DESIGN.md §3).
+ *   - Let the expanded batch be the B*K records in which row i*K + k is robot i's record with traj replaced by candidate k.
+ *     Candidate (i, k) gets, bit for bit, the wrench and status word hmpc_solve_device gives row i*K + k of the expanded
+ *     batch, in every size class and with hmpc_set_refinement on, and the cost hmpc_certify_device gives for that row and
+ *     that wrench.  Results: wrench [B][K][12N], status [B][K], cost NULL or double [B][K].
+ *   - cost: J = sum_k (x_k - traj_k)' S (x_k - traj_k) + u_k' Alpha_K u_k including the constant d'Sd, so candidates can be
+ *     ranked by it.  A candidate whose status code is not 0 has no trusted wrench, hence no trusted cost.
+ *   - Calls are cold: no working set is proposed or recorded, and the warm-start memory is not touched.
+ *   - A mask (NULL: every robot) skips robots with mask[i] == 0: their K rows of every output keep their bytes.
+ *   - Argument checks: a NULL context, records, traj, wrench or status pointer, K < 1 and B*K > capacity are HMPC_ERR_ARG;
+ *     B = 0 is a no-op.
+ *   hmpc_solve_device_multi: d_records B packed records, float traj and wrench, device mask.  One chain on `stream`, no
+ *                            host synchronisation.  Capturable.
+ *   hmpc_solve_batch_multi : in B update_data_t, host arrays, double wrenches (the solver's own: they round to the device
+ *                            call's floats).  In place when in, traj, wrench_out, status and cost_out lie in pinned ranges
+ *                            (hmpc_pin_host_buffer), else staged through the context's pinned memory; the same results.
+ *                            Its cost is hmpc_certify_batch's for the expanded row and the double wrench.  Returns
+ *                            HMPC_ERR_NOT_CONVERGED when a listed candidate did not reach a KKT point. */
+HMPC_EXTERNC int hmpc_solve_device_multi(hmpc_ctx* ctx, const void* d_records, int B, int K, const float* d_traj,
+                                         const unsigned char* d_mask, float* d_wrench, int* d_status, double* d_cost,
+                                         void* stream);
+HMPC_EXTERNC int hmpc_solve_batch_multi(hmpc_ctx* ctx, const struct update_data_t* in, int B, int K, const float* traj,
+                                        const unsigned char* mask, double* wrench_out, int* status, double* cost_out);
+/* test hook: 1 when the last hmpc_solve_batch_multi that launched ran in place, 0 when it staged, -1 before any */
+HMPC_EXTERNC int hmpc_debug_last_multi_in_place(void);
 /* The reference boundary warm-started: after hmpc_reference_set_warm_start(1), every update_problem_data proposes the
  * previous call's working set moved one step (a hmpc_solve_batch_warm with shift NULL on the one-robot context).
  * setup_problem with another dt, f_max or horizon forgets it.  Default 0: every tick a cold start, like the reference. */
@@ -444,7 +472,7 @@ HMPC_EXTERNC int hmpc_swing_device(hmpc_ctx* ctx, const struct hmpc_state_t* d_s
 /* CUDA graphs.  The device-resident calls can be recorded into a CUDA graph by stream capture (cudaStreamBeginCapture,
  * torch.cuda.graph, ...) on the stream they are given: hmpc_solve_device, hmpc_solve_device_ex, hmpc_solve_device_warm,
  * hmpc_solve_device_masked, hmpc_solve_states_device_masked, hmpc_prepare_device, hmpc_rollout_device, hmpc_swing_device,
- * hmpc_predict_device, hmpc_certify_device and hmpc_reset_warm_start.  Each
+ * hmpc_predict_device, hmpc_certify_device, hmpc_solve_device_multi and hmpc_reset_warm_start.  Each
  * launch of the graph gives the results an eager call on the same inputs gives, bit for bit.
  *   - A replay is a real call.  A captured warm solve proposes and records working sets, a captured rollout advances
  *     d_states and d_loop, a captured hmpc_reset_warm_start clears the working sets, every time the graph is launched.
@@ -456,7 +484,7 @@ HMPC_EXTERNC int hmpc_swing_device(hmpc_ctx* ctx, const struct hmpc_state_t* d_s
  *   - A call that returns an error while its stream is capturing may have recorded part of its work: end the capture
  *     and discard the graph.  Argument errors are found before anything is enqueued.
  * The host-buffer calls (hmpc_solve_batch, _ex, _warm, _masked, _states, _states_warm, _states_masked,
- * hmpc_solve_batch_sharded, hmpc_predict_batch, hmpc_certify_batch) and the reference boundary
+ * hmpc_solve_batch_sharded, hmpc_predict_batch, hmpc_certify_batch, hmpc_solve_batch_multi) and the reference boundary
  * (update_problem_data) wait for their own streams and cannot be captured. */
 
 /* Robots beyond the conditioning limit (INTEGRATION.md).  The fp64 sweep inversion of the solve is accurate up to a scaled
