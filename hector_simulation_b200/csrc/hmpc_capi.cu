@@ -146,6 +146,10 @@ struct hmpc_ctx {
   float* d_mq = nullptr;
   size_t mq_off[4] = {};
   unsigned char* h_multi = nullptr;  // pinned, max_batch x (row, traj, wrench, status, cost) of a staged hmpc_solve_batch_multi
+  // hmpc_solve_batch_states_multi (allocated by the first one): the candidates' trajectories [max_batch][12N], and pinned
+  // max_batch x (state, command, wrench, status, cost, best) of a staged call
+  float* d_smtraj = nullptr;
+  unsigned char* h_smulti = nullptr;
   int* d_ref = nullptr;            // host-buffer path: [NCHUNK][1 + max_batch] refinement list length + list
   unsigned char* d_rec = nullptr;
   unsigned char* d_out = nullptr;  // host-buffer path: result staging (rows())
@@ -314,6 +318,16 @@ int launch_prepare(const hmpc::PrepareArgs& pa, cudaStream_t st, bool pdl)
   return HMPC_OK;
 }
 
+// the trajectory preparation of a multi-command states call (hmpc_chain.h: prepare_traj_args) on one thread per (robot or
+// list entry, candidate) at most
+int launch_prepare_traj(const hmpc::PrepareTrajArgs& pa, cudaStream_t st, bool pdl)
+{
+  CK(launch_chain(hmpc::hmpc_prepare_traj_kernel, dim3(hmpc::prepare_grid(pa.batch * pa.K)), dim3(hmpc::PREPARE_THREADS), 0, st,
+                  pdl, pa.states, pa.batch, pa.K, pa.cmd, pa.N, pa.dtMPC, pa.traj, pa.list, pa.count));
+  CK(cudaGetLastError());
+  return HMPC_OK;
+}
+
 // the carry kernel (hmpc_chain.h: carry_grid): rows of `cur` the mask does not list get their bytes from `prev`
 int launch_carry(const unsigned char* mask, int batch, int N, const float* prev, float* cur, cudaStream_t st)
 {
@@ -353,6 +367,18 @@ int launch_multi_cost(const hmpc_ctx* c, const void* rows, hmpc::RowLayout lay, 
 {
   hmpc::hmpc_multi_cost_kernel<T><<<hmpc::multi_cost_grid((long long)B * K), hmpc::PREDICT_THREADS, 0, st>>>(
       static_cast<const unsigned char*>(rows), lay, B, K, c->horizon, c->cfg.dt, mask, traj, wrench, cost);
+  CK(cudaGetLastError());
+  return HMPC_OK;
+}
+
+// the pick kernel of a multi-command states call (hmpc_chain.h: pick_grid) over the B robots
+template <typename T>
+int launch_pick(const hmpc_ctx* c, void* records, int B, int K, const unsigned char* mask, const float* traj, const T* wrench,
+                const int* status, const double* cost, int* best, float* tau, cudaStream_t st)
+{
+  hmpc::hmpc_pick_kernel<T><<<hmpc::pick_grid(B), hmpc::PREDICT_THREADS, 0, st>>>(
+      static_cast<unsigned char*>(records), c->rec_stride, B, K, c->horizon, c->cfg.f_max, mask, traj, wrench, status, cost, best,
+      tau);
   CK(cudaGetLastError());
   return HMPC_OK;
 }
@@ -524,6 +550,8 @@ HMPC_EXTERNC void hmpc_destroy(hmpc_ctx* c)
   if (c->d_ref) cudaFree(c->d_ref);
   if (c->d_mq) cudaFree(c->d_mq);
   if (c->h_multi) cudaFreeHost(c->h_multi);
+  if (c->d_smtraj) cudaFree(c->d_smtraj);
+  if (c->h_smulti) cudaFreeHost(c->h_smulti);
   shard_release(c);
   if (c->d_ws) cudaFree(c->d_ws);
   if (c->d_shift) cudaFree(c->d_shift);
@@ -661,8 +689,11 @@ int enqueue_solve(hmpc_ctx* c, const hmpc::SolveIO& io, cudaStream_t st, const h
     CK(cudaGetLastError());
   }
   if (io.states) {
-    // the states chain: records of the listed robots (every robot without a mask) into io.records, read by class 0
+    // the states chain: records of the listed robots (every robot without a mask) into io.records, read by class 0; with
+    // commands, then their candidates' trajectories
     if (int rc = launch_prepare(hmpc::prepare_args(c->horizon, io, lists), st, pdl)) return rc;
+    if (mq && mq->cmd)
+      if (int rc = launch_prepare_traj(hmpc::prepare_traj_args(c->horizon, io, lists, *mq), st, pdl)) return rc;
   }
   const int items = mq ? io.batch * mq->K : io.batch;
   for (int i = 0; i < c->ncls; i++)
@@ -1126,6 +1157,129 @@ HMPC_EXTERNC int hmpc_solve_batch_multi(hmpc_ctx* c, const update_data_t* in, in
       if (HMPC_STATUS_CODE(status[r0 + k]) != 0) rc = HMPC_ERR_NOT_CONVERGED;
   }
   if (rc) g_err = "hmpc_solve_batch_multi: at least one candidate did not reach a KKT point (see status[])";
+  return rc;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// candidate commands per robot, from its state (hmpc_chain.h: PrepareTrajArgs)
+// ---------------------------------------------------------------------------------------------------
+static_assert(sizeof(hmpc_command_t) == 7 * 8 && offsetof(hmpc_state_t, state_des) == 32 * 8 &&
+                  offsetof(hmpc_state_t, world_position_desired) == 37 * 8 && offsetof(hmpc_command_t, world_position_desired) == 5 * 8,
+              "hmpc_command_t is the state's bytes [256, 312) (hmpc_prepare_traj_kernel)");
+
+// The chain of a multi-command states call on `io` (states, records, outputs, mask set) with K commands `cmd` and trajectory
+// buffer `traj`: preparation, classes, cost, pick.  T: the wrench's element type (float: io.wrench, double: io.wrench64).
+template <typename T>
+static int enqueue_states_multi(hmpc_ctx* c, const hmpc::SolveIO& io, int K, const hmpc_command_t* cmd, float* traj, double* cost,
+                                int* best, float* tau, cudaStream_t st)
+{
+  hmpc::MultiIO mq = multi_io(c, traj, K);
+  mq.cmd = reinterpret_cast<const double*>(cmd);
+  if (int rc = enqueue_solve(c, io, st, &mq)) return rc;
+  const T* w;
+  if constexpr (sizeof(T) == 4) w = io.wrench; else w = io.wrench64;
+  if (int rc = launch_multi_cost(c, io.records, hmpc::packed_rows(c->horizon), io.batch, K, io.mask, traj, w, cost, st)) return rc;
+  return launch_pick(c, const_cast<void*>(io.records), io.batch, K, io.mask, traj, w, io.status, cost, best, tau, st);
+}
+
+HMPC_EXTERNC int hmpc_solve_states_device_multi(hmpc_ctx* c, const hmpc_state_t* d_states, int B, int K, const hmpc_command_t* d_cmd,
+                                                const unsigned char* d_mask, double dtMPC, void* d_records, float* d_traj,
+                                                float* d_wrench, int* d_status, double* d_cost, int* d_best, float* d_tau,
+                                                void* stream)
+{
+  if (!c || !d_states || !d_cmd || !d_records || !d_traj || !d_wrench || !d_status || !d_cost || !d_best) {
+    g_err = "hmpc_solve_states_device_multi: null argument";
+    return HMPC_ERR_ARG;
+  }
+  if (int rc = check_multi(c, B, K, "hmpc_solve_states_device_multi")) return rc;
+  if (B == 0) return HMPC_OK;
+  if (int rc = check_device_records(c, d_records, B, "hmpc_solve_states_device_multi")) return rc;
+  hmpc::SolveIO io = device_call(c, d_records, B, d_wrench, d_status, nullptr, false);
+  io.mask = d_mask;
+  io.states = d_states;
+  io.dt_mpc = dtMPC;
+  return enqueue_states_multi<float>(c, io, K, d_cmd, d_traj, d_cost, d_best, d_tau, static_cast<cudaStream_t>(stream));
+}
+
+namespace { int g_states_multi_in_place = -1; }
+HMPC_EXTERNC int hmpc_debug_last_states_multi_in_place(void) { return g_states_multi_in_place; }
+
+// The chain of hmpc_solve_states_device_multi on the context's records and trajectory buffer, with double wrenches: on the
+// caller's arrays when they are pinned (the kernels read the states and commands and store the results where they lie),
+// else on copies of the listed robots' rows in h_smulti, which the kernels read and write mapped.  Torques go through the
+// pinned result staging (h_out) as float rows and are widened here, as in the other host calls.
+HMPC_EXTERNC int hmpc_solve_batch_states_multi(hmpc_ctx* c, const hmpc_state_t* in, int B, int K, const hmpc_command_t* cmd,
+                                               const unsigned char* mask, double dtMPC, double* wrench_out, int* status,
+                                               double* cost_out, int* best, double* tau_out)
+{
+  if (!c || !in || !cmd || !wrench_out || !status || !cost_out || !best) {
+    g_err = "hmpc_solve_batch_states_multi: null argument";
+    return HMPC_ERR_ARG;
+  }
+  if (int rc = check_multi(c, B, K, "hmpc_solve_batch_states_multi")) return rc;
+  if (B == 0) return HMPC_OK;
+  if (mask && std::all_of(mask, mask + B, [](unsigned char m) { return m == 0; })) return HMPC_OK;
+  CK(cudaSetDevice(c->device));
+  const size_t nw = (size_t)12 * c->horizon, R = (size_t)B * K, mb = (size_t)c->max_batch;
+  if (!c->d_smtraj) CK(cudaMalloc(&c->d_smtraj, mb * nw * sizeof(float)));
+  const unsigned char* m = nullptr;
+  if (mask) {
+    memcpy(c->h_mask, mask, (size_t)B);  // pinned: the selection kernel, the cost and the pick kernel read it mapped
+    m = c->h_mask;
+  }
+  auto listed = [&](int i) { return !mask || mask[i] != 0; };
+  const bool in_place = c->pinned(in, (size_t)B * sizeof(hmpc_state_t)) && c->pinned(cmd, R * sizeof(hmpc_command_t)) &&
+                        c->pinned(wrench_out, R * nw * sizeof(double)) && c->pinned(status, R * sizeof(int)) &&
+                        c->pinned(cost_out, R * sizeof(double)) && c->pinned(best, (size_t)B * sizeof(int));
+  g_states_multi_in_place = in_place ? 1 : 0;
+  const hmpc_state_t* states = in;
+  const hmpc_command_t* cm = cmd;
+  double* w = wrench_out;
+  int* st = status;
+  double* cost = cost_out;
+  int* bst = best;
+  if (!in_place) {  // [max_batch states | max_batch commands | max_batch x 12N wrench doubles | cost doubles | status ints | best ints]
+    if (!c->h_smulti)
+      CK(cudaMallocHost(&c->h_smulti, mb * (sizeof(hmpc_state_t) + sizeof(hmpc_command_t) + nw * sizeof(double) + sizeof(double) +
+                                            2 * sizeof(int))));
+    hmpc_state_t* hs = reinterpret_cast<hmpc_state_t*>(c->h_smulti);
+    hmpc_command_t* hc = reinterpret_cast<hmpc_command_t*>(hs + mb);
+    double* hw = reinterpret_cast<double*>(hc + mb);
+    double* hcost = hw + mb * nw;
+    int* hst = reinterpret_cast<int*>(hcost + mb);
+    for (int i = 0; i < B; i++)
+      if (listed(i)) {
+        hs[i] = in[i];
+        memcpy(hc + (size_t)i * K, cmd + (size_t)i * K, K * sizeof(hmpc_command_t));
+      }
+    states = hs, cm = hc, w = hw, st = hst, cost = hcost, bst = hst + mb;
+  }
+  float* tau = tau_out ? c->rows(c->h_out, 0, c->max_batch).tau : nullptr;  // pinned, written mapped
+  hmpc::SolveIO io;
+  io.states = states;
+  io.dt_mpc = dtMPC;
+  io.records = c->d_rec;
+  io.batch = B;
+  io.wrench64 = w;
+  io.status = st;
+  io.mask = m;
+  if (int rc = enqueue_states_multi<double>(c, io, K, cm, c->d_smtraj, cost, bst, tau, c->stream)) return rc;
+  CK(cudaStreamSynchronize(c->stream));
+  int rc = HMPC_OK;
+  for (int i = 0; i < B; i++) {
+    if (!listed(i)) continue;
+    const size_t r0 = (size_t)i * K;
+    if (!in_place) {
+      memcpy(wrench_out + r0 * nw, w + r0 * nw, K * nw * sizeof(double));
+      memcpy(status + r0, st + r0, K * sizeof(int));
+      memcpy(cost_out + r0, cost + r0, K * sizeof(double));
+      best[i] = bst[i];
+    }
+    if (tau_out)
+      for (int j = 0; j < 10; j++) tau_out[(size_t)i * 10 + j] = (double)tau[(size_t)i * 10 + j];
+    if (best[i] < 0) rc = HMPC_ERR_NOT_CONVERGED;
+  }
+  if (rc) g_err = "hmpc_solve_batch_states_multi: no candidate of at least one robot reached a KKT point (see best[], status[])";
   return rc;
 }
 

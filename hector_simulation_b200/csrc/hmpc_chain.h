@@ -364,10 +364,13 @@ inline KernelArgs launch_args(const SolverSettings& S, int N, int ncls, int cls,
 // classes (plan_classes(..., mq = true)), K candidate trajectories per robot (traj [batch][K][12N]) and results in rows
 // i*K + k of io.wrench / io.wrench64 / io.status.  Calls are cold: no working set is proposed or recorded, and no torques.
 // scratch[c]: class c's scratch (REFINE_CLASS: scratch[3]), mq_scratch_floats(N) floats per CTA of its launch.
+// cmd: a multi-command states call (hmpc_solve_states_device_multi, below): [batch][K] commands, 7 doubles each; the chain's
+// preparation writes traj from them.
 struct MultiIO {
   const float* traj = nullptr;
   int K = 1;
   float* scratch[4] = {};
+  const double* cmd = nullptr;
 };
 inline KernelArgs multi_launch_args(const SolverSettings& S, int N, int ncls, int cls, const ClassCfg& k, const SolveIO& io,
                                     const ChainLists& lists, const MultiIO& mq)
@@ -392,6 +395,41 @@ inline int multi_cost_grid(long long nrows)
 {
   constexpr int warps = PREDICT_THREADS / 32;
   return (int)((nrows + warps - 1) / warps);
+}
+
+// A multi-command states call (hmpc_solve_states_device_multi, hmpc_solve_batch_states_multi), one chain on one stream:
+//   [the selection kernel over the mask]
+//   -> the preparation (hmpc_prepare_kernel, prepare_args) of the listed robots' records into io.records, as in the states
+//      chain; its traj is the state's own command's, which the pick kernel replaces
+//   -> the trajectories (hmpc_prepare_traj_kernel) of their K commands mq.cmd into mq.traj [batch][K][12N],
+//      prepare_grid(io.batch * K) CTAs of PREPARE_THREADS, one thread per (robot, candidate) over class 0's list (every
+//      robot without a mask)
+//   -> the multi-query classes over those records and trajectories (multi_launch_args)
+//   -> the cost kernel (hmpc_multi_cost_kernel, multi_cost_grid(io.batch * K))
+//   -> the pick kernel (hmpc_pick_kernel, pick_grid(io.batch)): best, torques, and the chosen trajectory into the record.
+// The two preparation kernels are links of the PDL chain (each waits for its predecessor and the previous call before it
+// reads or stores; class 0 waits for the second); the cost and pick kernels follow in plain stream order.
+struct PrepareTrajArgs {
+  const unsigned char* states;
+  int batch, K;
+  const double* cmd;
+  int N;
+  double dtMPC;
+  float* traj;
+  const int* list;
+  const int* count;
+};
+inline PrepareTrajArgs prepare_traj_args(int N, const SolveIO& io, const ChainLists& lists, const MultiIO& mq)
+{
+  const PrepareArgs pa = prepare_args(N, io, lists);
+  return PrepareTrajArgs{pa.states, pa.batch, mq.K, mq.cmd, N, pa.dtMPC, const_cast<float*>(mq.traj),  // (written here, read
+                         pa.list, pa.count};                                                              // by the classes)
+}
+// the pick launch: one warp per robot
+inline int pick_grid(int batch)
+{
+  constexpr int warps = PREDICT_THREADS / 32;
+  return (batch + warps - 1) / warps;
 }
 
 }  // namespace hmpc

@@ -561,6 +561,36 @@ __device__ inline double leg_torque(const double* q5, int leg, int j, const doub
   return t;
 }
 
+// Row f-2: the feed-forward torque of joint j of leg `leg`, tau = J_force_moment^T * f_ff with f_ff = -rBody [F; M] of the leg's
+// first-step wrench w [6] (ConvexMPCLocomotion.cpp:419-440, LegController.cpp:57-63); a swing leg (w null) gets no
+// feed-forward force.  q10: a record's 10 joint-angle floats, quat: its 4 quaternion floats.  W: the wrench's element type
+// (rounded to float first).  The pick kernel (hmpc_pick_kernel) runs it; it states the solve kernel's torque epilogue (stage
+// 6) operation for operation, which keeps its own inline copy so that its instruction schedule stays as it is.
+template <typename W>
+__device__ __forceinline__ float joint_torque(const float* q10, const float* quat, int leg, int j, const W* w)
+{
+  const double PI = 3.14159265359;
+  double q5[5];
+#pragma unroll
+  for (int i = 0; i < 5; i++) q5[i] = (double)q10[5 * leg + i];
+  q5[2] -= 0.3 * PI;  // undo the caller's second offset: LegController's own angles
+  q5[3] += 0.6 * PI;
+  q5[4] -= 0.3 * PI;
+  const double qw = quat[0], qx = quat[1], qy = quat[2], qz = quat[3];
+  const double R[9] = {1 - 2 * (qy * qy + qz * qz), 2 * (qx * qy - qw * qz), 2 * (qx * qz + qw * qy),
+                       2 * (qx * qy + qw * qz), 1 - 2 * (qx * qx + qz * qz), 2 * (qy * qz - qw * qx),
+                       2 * (qx * qz - qw * qy), 2 * (qy * qz + qw * qx), 1 - 2 * (qx * qx + qy * qy)};
+  double fw[6] = {0, 0, 0, 0, 0, 0};
+  if (w) {
+#pragma unroll
+    for (int r = 0; r < 3; r++) {  // rBody = R^T
+      fw[r] = -(R[0 * 3 + r] * (double)(float)w[0] + R[1 * 3 + r] * (double)(float)w[1] + R[2 * 3 + r] * (double)(float)w[2]);
+      fw[3 + r] = -(R[0 * 3 + r] * (double)(float)w[3] + R[1 * 3 + r] * (double)(float)w[4] + R[2 * 3 + r] * (double)(float)w[5]);
+    }
+  }
+  return (float)leg_torque(q5, leg, j, fw);
+}
+
 // fast fp64 reciprocal: MUFU.RCP64H seed (relative error 9.9e-7 on the H100, tests/tools/ubench.cu) + two Newton steps:
 // identical to the IEEE quotient on 5e7 probe values, a third step changes nothing; the IEEE division sequence is ~6x
 // the instructions and the reciprocals sit on the critical chains of the tile inversions and the Schur sweeps
@@ -713,6 +743,63 @@ __global__ void hmpc_prepare_kernel(const unsigned char* states, int batch, int 
   unsigned char* g = records + (size_t)i * rec_stride + (54 + 12 * N) * 4;
   for (int e = 0; e < 2 * N; e++) g[e] = gait[e];
   for (int e = (54 + 12 * N) * 4 + 2 * N; e < rec_stride; e++) records[(size_t)i * rec_stride + e] = 0;
+}
+
+// The reference trajectory (:331-399) of one command into out [12N]: R the body -> world rotation, pos and rpy the state's,
+// sd (roll, pitch, body vx, vy, yaw rate) and wpd [2] the command (hmpc_state_t::state_des, world_position_desired).  The
+// operations of hmpc_prepare_kernel's trajectory block, one for one and explicitly rounded, so a candidate's trajectory is
+// the traj that kernel writes for a state with that command, bit for bit.  (hmpc_prepare_kernel keeps its own inline copy:
+// calling this function from it changed that kernel's register assignment and instruction schedule.)
+__device__ __forceinline__ void prepare_traj(const double* R, const double* pos, const double* rpy, const double* sd,
+                                             const double* wpd, int N, double dtMPC, float* out)
+{
+  const double yaw = rpy[2];
+  const double vdr[3] = {sd[2], sd[3], 0.0};
+  double vdw[3];
+  for (int a = 0; a < 3; a++) vdw[a] = DA(DA(DM(R[a * 3], vdr[0]), DM(R[a * 3 + 1], vdr[1])), DM(R[a * 3 + 2], vdr[2]));
+  const double mpe = .05;
+  double xS = wpd[0], yS = wpd[1];
+  if (DS(xS, pos[0]) > mpe) xS = DA(pos[0], mpe);
+  if (DS(pos[0], xS) > mpe) xS = DS(pos[0], mpe);
+  if (DS(yS, pos[1]) > mpe) yS = DA(pos[1], mpe);
+  if (DS(pos[1], yS) > mpe) yS = DS(pos[1], mpe);
+  const double ti[12] = {sd[0], sd[1], 0.0, xS, yS, 0.55, 0, 0, sd[4], vdw[0], vdw[1], 0};
+  for (int st = 0; st < N; st++) {
+    double tr[12];
+    for (int j = 0; j < 12; j++) tr[j] = ti[j];
+    if (st == 0) {
+      tr[0] = rpy[0]; tr[1] = rpy[1]; tr[2] = rpy[2];
+      tr[3] = pos[0]; tr[4] = pos[1]; tr[5] = pos[2];
+    } else {
+      const double idt = DM((double)st, dtMPC);
+      tr[3] = DA(vdw[0] == 0 ? ti[3] : pos[0], DM(idt, vdw[0]));
+      tr[4] = DA(vdw[1] == 0 ? ti[4] : pos[1], DM(idt, vdw[1]));
+      tr[2] = (sd[4] == 0) ? ti[2] : DA(yaw, DM(idt, sd[4]));
+    }
+    for (int j = 0; j < 12; j++) out[12 * st + j] = (float)tr[j];
+  }
+}
+
+// The trajectories of a multi-command states call (hmpc_solve_states_device_multi): for each robot the chain's
+// hmpc_prepare_kernel prepares, the reference trajectories of its K commands cmd[i][k] (hmpc_command_t: 7 doubles, laid out
+// like the state's bytes [256, 312)) into traj[i][k] [12N].  One thread per (robot, candidate); `list` / `count` as in
+// hmpc_prepare_kernel, with K threads per list entry.  Launch shape: hmpc_chain.h, prepare_grid(batch * K).
+__global__ void hmpc_prepare_traj_kernel(const unsigned char* states, int batch, int K, const double* cmd, int N, double dtMPC,
+                                         float* traj, const int* list, const int* count)
+{
+  pdl_trigger();  // class 0 may become resident; it waits for this kernel before it reads the trajectories
+  pdl_wait();     // (the list, and the previous call's readers of traj, as in hmpc_prepare_kernel)
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (list ? *count : batch) * K) return;
+  const int e = t / K, k = t % K;
+  const int i = list ? list[e] : e;
+  const double* s = reinterpret_cast<const double*>(states + (size_t)i * 352);
+  const double e0 = s[6], e1 = s[7], e2 = s[8], e3 = s[9];  // the quaternion: hmpc_prepare_kernel's body -> world rotation
+  const double R[9] = {DS(1.0, DM(2.0, DA(DM(e2, e2), DM(e3, e3)))), DM(2.0, DS(DM(e1, e2), DM(e0, e3))), DM(2.0, DA(DM(e1, e3), DM(e0, e2))),
+                       DM(2.0, DA(DM(e1, e2), DM(e0, e3))), DS(1.0, DM(2.0, DA(DM(e1, e1), DM(e3, e3)))), DM(2.0, DS(DM(e2, e3), DM(e0, e1))),
+                       DM(2.0, DS(DM(e1, e3), DM(e0, e2))), DM(2.0, DA(DM(e2, e3), DM(e0, e1))), DS(1.0, DM(2.0, DA(DM(e1, e1), DM(e2, e2))))};
+  const size_t q = (size_t)i * K + k;
+  prepare_traj(R, s, s + 13, cmd + q * 7, cmd + q * 7 + 5, N, dtMPC, traj + q * 12 * N);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -3039,6 +3126,54 @@ __global__ void __launch_bounds__(PREDICT_THREADS) hmpc_multi_cost_kernel(const 
   }
   const double J = cost_total(c);
   if (lane == 0) cost[q] = J;
+}
+
+// ------------------------------------------------------------------------------------------------
+// The pick of a multi-command states call (hmpc_solve_states_device_multi), behind its cost kernel: per robot i, best[i] =
+// the k with the smallest cost[i][k] among the candidates whose status code is 0 and whose cost is finite, the lowest such k
+// on ties, or -1 when there is none.  Then robot i's torque row: joint_torque on the record's joint angles and quaternion and
+// the chosen candidate's step-0 wrench, what the solve's epilogue gives that candidate's expanded row (zeros for -1).  Last
+// the record's traj is set to the chosen candidate's, traj[i][best] (candidate 0 for -1), so the record is the one
+// hmpc_prepare_kernel writes for the chosen command.  One warp per robot; robots with mask[i] == 0 (mask non-null) are
+// skipped; tau may be null.  T: the wrench's element type.  Launch shape: hmpc_chain.h, pick_grid.
+// ------------------------------------------------------------------------------------------------
+template <typename T>
+__global__ void __launch_bounds__(PREDICT_THREADS) hmpc_pick_kernel(unsigned char* records, int rec_stride, int batch, int K,
+                                                                     int N, float f_max, const unsigned char* mask,
+                                                                     const float* traj, const T* wrench, const int* status,
+                                                                     const double* cost, int* best, float* tau)
+{
+  constexpr int NW = PREDICT_THREADS / 32;
+  const int lane = threadIdx.x & 31;
+  const int i = blockIdx.x * NW + (threadIdx.x >> 5);
+  if (i >= batch || (mask && mask[i] == 0)) return;  // (the whole warp)
+  const size_t r0 = (size_t)i * K;
+  double bc = 0.0;
+  int bk = -1;
+  for (int k = lane; k < K; k += 32)  // (ascending k: a tie keeps the lower one)
+    if ((status[r0 + k] & 0xff) == 0 && finite64(cost[r0 + k]) && (bk < 0 || cost[r0 + k] < bc)) bc = cost[r0 + k], bk = k;
+  for (int o = 16; o > 0; o >>= 1) {
+    const double oc = __shfl_xor_sync(0xffffffffu, bc, o);
+    const int ok = __shfl_xor_sync(0xffffffffu, bk, o);
+    if (ok >= 0 && (bk < 0 || oc < bc || (oc == bc && ok < bk))) bc = oc, bk = ok;
+  }
+  float* f = reinterpret_cast<float*>(records + (size_t)i * rec_stride);
+  const float* src = traj + (r0 + (bk < 0 ? 0 : bk)) * 12 * N;
+  if (tau && lane < 10) {
+    float t = 0.f;
+    if (bk >= 0) {
+      const int leg = lane / 5, j = lane % 5;
+      const float ub = FM(f_max, (float)(records + (size_t)i * rec_stride + (54 + 12 * N) * 4)[leg]);  // step 0's gait byte
+      const T* w = wrench + (r0 + bk) * 12 * N;
+      T w6[6];
+      for (int c = 0; c < 6; c++) w6[c] = w[col12_of(leg, c)];
+      t = joint_torque(f + 19, f + 6, leg, j, (ub < 0.0001f && ub > -0.0001f) ? nullptr : w6);  // (stage 1's swing test)
+    }
+    tau[(size_t)i * 10 + lane] = t;
+  }
+  __syncwarp();  // (the torques read the record's floats 6-28, the copy below writes 54 on)
+  for (int e = lane; e < 12 * N; e += 32) f[54 + e] = src[e];
+  if (lane == 0) best[i] = bk;
 }
 
 }  // namespace hmpc

@@ -12,7 +12,7 @@ import os
 
 import numpy as np
 
-from .scenarios import STATE_DTYPE, UPDATE_DTYPE
+from .scenarios import COMMAND_DTYPE, STATE_DTYPE, UPDATE_DTYPE
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libhector_mpc_b200.so")
@@ -36,6 +36,7 @@ EXPORTS = [
     "hmpc_solve_batch_sharded_warm", "hmpc_solve_batch_states_sharded_warm",
     "hmpc_predict_device", "hmpc_predict_batch", "hmpc_certify_device", "hmpc_certify_batch",
     "hmpc_solve_device_multi", "hmpc_solve_batch_multi",
+    "hmpc_solve_states_device_multi", "hmpc_solve_batch_states_multi",
 ]
 # hmpc_certificate_t, and its flag bits (include/hector_mpc_b200.h)
 CERTIFICATE_DTYPE = np.dtype([("cost", "<f8"), ("stationarity", "<f8"), ("primal", "<f8"), ("complementarity", "<f8"),
@@ -157,6 +158,12 @@ def lib() -> ctypes.CDLL:
         L.hmpc_solve_device_multi.restype = ctypes.c_int
         L.hmpc_solve_batch_multi.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 5
         L.hmpc_solve_batch_multi.restype = ctypes.c_int
+        L.hmpc_solve_states_device_multi.argtypes = ([ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 2
+                                                     + [ctypes.c_double] + [ctypes.c_void_p] * 8)
+        L.hmpc_solve_states_device_multi.restype = ctypes.c_int
+        L.hmpc_solve_batch_states_multi.argtypes = ([ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 2
+                                                    + [ctypes.c_double] + [ctypes.c_void_p] * 5)
+        L.hmpc_solve_batch_states_multi.restype = ctypes.c_int
         _lib = L
     return _lib
 
@@ -639,6 +646,57 @@ class BatchedMPC:
                                             st.ctypes.data, c.ctypes.data if c is not None else None),
                allow_not_converged=not strict)
         return w, st, c
+
+    def solve_states_device_multi(self, d_states, B: int, d_cmd, d_records, d_traj, d_wrench, d_status, d_cost, d_best,
+                                  d_tau=None, d_mask=None, stream=None, dt_mpc: float = 0.04) -> None:
+        """Robot i's MPC for K candidate commands from its state, the cheapest converged one picked on the device
+        (hmpc_solve_states_device_multi).  torch CUDA tensors: d_states uint8 [B,352], d_cmd uint8 [B,K,56] or f64 [B,K,7]
+        (COMMAND_DTYPE: state_des, world_position_desired); d_records uint8 [B,stride] receives the record of the chosen
+        command, d_traj f32 [B,K,12N] the candidates' trajectories; results d_wrench f32 [B,K,12N], d_status i32 [B,K], d_cost
+        f64 [B,K], d_best i32 [B] (-1: no candidate converged), d_tau f32 [B,10] or None (the chosen candidate's torques).
+        Each equals the expanded batch's prepare_device / solve_device_ex / certify_device, bit for bit.  `d_mask` bool or
+        uint8 [B] or None: unlisted robots' rows keep their bytes.  Cold, enqueued on the current stream, capturable."""
+        import torch
+
+        K = d_traj.shape[1]
+        st = torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+        _check(lib().hmpc_solve_states_device_multi(self._h, d_states.data_ptr(), B, K, d_cmd.data_ptr(),
+                                                    d_mask.data_ptr() if d_mask is not None else None, dt_mpc,
+                                                    d_records.data_ptr(), d_traj.data_ptr(), d_wrench.data_ptr(),
+                                                    d_status.data_ptr(), d_cost.data_ptr(), d_best.data_ptr(),
+                                                    d_tau.data_ptr() if d_tau is not None else None, ctypes.c_void_p(st)))
+
+    def solve_batch_states_multi(self, states: np.ndarray, cmd: np.ndarray, mask=None, torques: bool = True,
+                                 strict: bool = True, out=None, dt_mpc: float = 0.04):
+        """solve_states_device_multi from host buffers (hmpc_solve_batch_states_multi): `states` STATE_DTYPE [B], `cmd`
+        COMMAND_DTYPE [B,K] -> (wrench f64 [B,K,12N], status i32 [B,K], cost f64 [B,K], best i32 [B], tau f64 [B,10] or
+        None).  `out=(wrench, status, cost, best, tau)` reuses the caller's arrays (tau may be None); in place when states,
+        cmd and every output but tau are pinned (pin()).  With a mask only listed robots' rows are written.  strict: raise
+        when a listed robot has no converged candidate (best == -1)."""
+        states = np.ascontiguousarray(states, dtype=STATE_DTYPE)
+        cmd = np.ascontiguousarray(cmd, dtype=COMMAND_DTYPE)
+        B, N = states.shape[0], self.horizon
+        assert cmd.ndim == 2 and cmd.shape[0] == B
+        K = cmd.shape[1]
+        if out is None:
+            out = (np.zeros((B, K, 12 * N), np.float64), np.zeros((B, K), np.int32), np.zeros((B, K), np.float64),
+                   np.zeros(B, np.int32), np.zeros((B, 10), np.float64) if torques else None)
+        w, st, c, best, tau = out
+        assert w.dtype == np.float64 and w.shape == (B, K, 12 * N) and w.flags.c_contiguous
+        assert st.dtype == np.int32 and st.shape == (B, K) and st.flags.c_contiguous
+        assert c.dtype == np.float64 and c.shape == (B, K) and c.flags.c_contiguous
+        assert best.dtype == np.int32 and best.shape == (B,) and best.flags.c_contiguous
+        assert tau is None or (tau.dtype == np.float64 and tau.shape == (B, 10) and tau.flags.c_contiguous)
+        m = None
+        if mask is not None:
+            mask = np.ascontiguousarray(np.asarray(mask) != 0).view(np.uint8)
+            assert mask.shape == (B,)
+            m = mask.ctypes.data
+        _check(lib().hmpc_solve_batch_states_multi(self._h, states.ctypes.data, B, K, cmd.ctypes.data, m, dt_mpc,
+                                                   w.ctypes.data, st.ctypes.data, c.ctypes.data, best.ctypes.data,
+                                                   tau.ctypes.data if tau is not None else None),
+               allow_not_converged=not strict)
+        return w, st, c, best, tau
 
     def assemble_device(self, d_records, B: int, stream=None) -> dict:
         """Parity hook: un-reduced fp32 QP data of B packed records (torch tensors on the GPU)."""

@@ -192,6 +192,26 @@ STATE_DTYPE = np.dtype([("position", "<f8", 3), ("vWorld", "<f8", 3), ("orientat
 assert STATE_DTYPE.itemsize == 352
 
 
+# numpy mirror of `hmpc_command_t` (include/hector_mpc_b200.h): the command part of a state, its bytes [256, 312)
+COMMAND_DTYPE = np.dtype([("state_des", "<f8", 5), ("world_position_desired", "<f8", 2)])
+assert COMMAND_DTYPE.itemsize == 56
+
+
+def command_candidates(states: np.ndarray, K: int, seed: int) -> np.ndarray:
+    """COMMAND_DTYPE [B, K]: K candidate commands per state for hmpc_solve_states_device_multi.  Candidate 0 is the state's
+    own command; the others change the body velocity (±0.3 m/s forward, ±0.15 m/s sideways), the yaw rate (±0.4 rad/s) and
+    the roll / pitch set-points (±0.05 rad) by seeded uniform amounts, enough to move the optimum and often its active set."""
+    rng = np.random.default_rng(seed)
+    B = len(states)
+    cmd = np.zeros((B, K), COMMAND_DTYPE)
+    cmd["state_des"] = states["state_des"][:, None, :]
+    cmd["world_position_desired"] = states["world_position_desired"][:, None, :]
+    if K > 1:
+        scale = np.array([0.05, 0.05, 0.3, 0.15, 0.4])
+        cmd["state_des"][:, 1:] += rng.uniform(-1.0, 1.0, (B, K - 1, 5)) * scale
+    return cmd
+
+
 def to_state(b: dict, horizon: int, out: np.ndarray | None = None) -> np.ndarray:
     """The caller-side state of one robot (row f-1 input) for the same tick as `to_record(b)`."""
     st = np.zeros((), dtype=STATE_DTYPE) if out is None else out

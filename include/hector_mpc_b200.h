@@ -389,6 +389,48 @@ HMPC_EXTERNC int hmpc_solve_batch_multi(hmpc_ctx* ctx, const struct update_data_
                                         const unsigned char* mask, double* wrench_out, int* status, double* cost_out);
 /* test hook: 1 when the last hmpc_solve_batch_multi that launched ran in place, 0 when it staged, -1 before any */
 HMPC_EXTERNC int hmpc_debug_last_multi_in_place(void);
+/* Candidate commands per robot, from its state: robot i's MPC solved for K commands cmd[i][k] at once, the cheapest
+ * converged one picked on the device.  A command is the part of hmpc_state_t the reference trajectory is built from
+ * (ConvexMPCLocomotion.cpp:331-399); every other field of the state is shared by the K candidates.  The chain prepares robot
+ * i's record once and its K trajectories, then runs hmpc_solve_device_multi's solve and cost on them, then a pick kernel
+ * (DESIGN.md §3).
+ *   - Let the expanded state batch be the B*K states in which row i*K + k is state i with its 56 command bytes replaced by
+ *     cmd[i][k].  Bit for bit, in every size class and with hmpc_set_refinement on:
+ *       traj[i][k]          the traj hmpc_prepare_device writes for expanded row i*K + k;
+ *       wrench[i][k],       what hmpc_solve_device gives the expanded prepared row (hmpc_solve_device_multi on robot i's record
+ *       status[i][k]        with those K trajectories);
+ *       cost[i][k]          what hmpc_certify_device reports as the cost of that row and wrench;
+ *       best[i]             the k of the smallest cost among the candidates with status code 0 and a finite cost, the lowest k
+ *                           on ties; -1 when there is none;
+ *       tau[i]              the torque row hmpc_solve_device_ex gives expanded row i*K + best[i]; zeros when best[i] = -1;
+ *       records row i       the record hmpc_prepare_device writes for expanded row i*K + best[i] (i*K when best[i] = -1), so
+ *                           hmpc_predict_device / hmpc_certify_device on (records, the chosen wrench) work directly.
+ *   - Calls are cold: no working set is proposed or recorded, and the warm-start memory is not touched.
+ *   - A mask (NULL: every robot) skips robots with mask[i] == 0: every output row of theirs keeps its bytes, records
+ *     included.
+ *   - Argument checks: a NULL context or required pointer (d_mask / mask and d_tau / tau_out may be NULL), K < 1 and
+ *     B*K > capacity are HMPC_ERR_ARG; B = 0 is a no-op.
+ *   hmpc_solve_states_device_multi: device arrays; d_records [B][hmpc_record_bytes] (16-byte aligned), d_traj float
+ *                            [B][K][12N], d_wrench float [B][K][12N], d_status [B][K], d_cost [B][K], d_best [B], d_tau float
+ *                            [B][10] or NULL.  One chain on `stream`, no host synchronisation.  Capturable.
+ *   hmpc_solve_batch_states_multi: host arrays, double wrenches and torques (the solver's own: they round to the device
+ *                            call's floats).  In place when in, cmd, wrench_out, status, cost_out and best lie in pinned ranges
+ *                            (hmpc_pin_host_buffer), else staged through the context's pinned memory; the same results.  The
+ *                            records and trajectories stay in the context.  Returns HMPC_ERR_NOT_CONVERGED when a listed robot
+ *                            has best == -1. */
+struct hmpc_command_t {            /* bytes [256, 312) of hmpc_state_t, same order */
+  double state_des[5];             /* roll, pitch, body vx, vy, yaw rate */
+  double world_position_desired[2];
+};
+HMPC_EXTERNC int hmpc_solve_states_device_multi(hmpc_ctx* ctx, const struct hmpc_state_t* d_states, int B, int K,
+                                                const struct hmpc_command_t* d_cmd, const unsigned char* d_mask, double dtMPC,
+                                                void* d_records, float* d_traj, float* d_wrench, int* d_status, double* d_cost,
+                                                int* d_best, float* d_tau, void* stream);
+HMPC_EXTERNC int hmpc_solve_batch_states_multi(hmpc_ctx* ctx, const struct hmpc_state_t* in, int B, int K,
+                                               const struct hmpc_command_t* cmd, const unsigned char* mask, double dtMPC,
+                                               double* wrench_out, int* status, double* cost_out, int* best, double* tau_out);
+/* test hook: 1 when the last hmpc_solve_batch_states_multi that launched ran in place, 0 when it staged, -1 before any */
+HMPC_EXTERNC int hmpc_debug_last_states_multi_in_place(void);
 /* The reference boundary warm-started: after hmpc_reference_set_warm_start(1), every update_problem_data proposes the
  * previous call's working set moved one step (a hmpc_solve_batch_warm with shift NULL on the one-robot context).
  * setup_problem with another dt, f_max or horizon forgets it.  Default 0: every tick a cold start, like the reference. */
@@ -472,7 +514,8 @@ HMPC_EXTERNC int hmpc_swing_device(hmpc_ctx* ctx, const struct hmpc_state_t* d_s
 /* CUDA graphs.  The device-resident calls can be recorded into a CUDA graph by stream capture (cudaStreamBeginCapture,
  * torch.cuda.graph, ...) on the stream they are given: hmpc_solve_device, hmpc_solve_device_ex, hmpc_solve_device_warm,
  * hmpc_solve_device_masked, hmpc_solve_states_device_masked, hmpc_prepare_device, hmpc_rollout_device, hmpc_swing_device,
- * hmpc_predict_device, hmpc_certify_device, hmpc_solve_device_multi and hmpc_reset_warm_start.  Each
+ * hmpc_predict_device, hmpc_certify_device, hmpc_solve_device_multi, hmpc_solve_states_device_multi and
+ * hmpc_reset_warm_start.  Each
  * launch of the graph gives the results an eager call on the same inputs gives, bit for bit.
  *   - A replay is a real call.  A captured warm solve proposes and records working sets, a captured rollout advances
  *     d_states and d_loop, a captured hmpc_reset_warm_start clears the working sets, every time the graph is launched.
@@ -484,7 +527,8 @@ HMPC_EXTERNC int hmpc_swing_device(hmpc_ctx* ctx, const struct hmpc_state_t* d_s
  *   - A call that returns an error while its stream is capturing may have recorded part of its work: end the capture
  *     and discard the graph.  Argument errors are found before anything is enqueued.
  * The host-buffer calls (hmpc_solve_batch, _ex, _warm, _masked, _states, _states_warm, _states_masked,
- * hmpc_solve_batch_sharded, hmpc_predict_batch, hmpc_certify_batch, hmpc_solve_batch_multi) and the reference boundary
+ * hmpc_solve_batch_sharded, hmpc_predict_batch, hmpc_certify_batch, hmpc_solve_batch_multi, hmpc_solve_batch_states_multi)
+ * and the reference boundary
  * (update_problem_data) wait for their own streams and cannot be captured. */
 
 /* Robots beyond the conditioning limit (INTEGRATION.md).  The fp64 sweep inversion of the solve is accurate up to a scaled
